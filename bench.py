@@ -27,7 +27,7 @@ scaling.  One step = one pass of the hot path over the whole batch of synthetic 
 
 ``--impl reference`` prints the CPU arm as its own line (rank 0 only under torchrun).
 ``--workload encode`` measures the chunk-embedding forward pass (configs[1]) instead; see bench_encode.py.
-Nothing here reads /root/reference.
+Nothing here reads the reference checkout.
 """
 from __future__ import annotations
 
@@ -73,7 +73,8 @@ def parse():
     ap.add_argument("--parity-queries", type=int, default=256,
                     help="queries compared with the CPU oracle over the full corpus after timing (0 = off)")
     ap.add_argument("--dense-kernel", type=int, default=0,
-                    help="0 auto, 1 simt, 2 tcgen05 SS, 3 tcgen05 TS (N=64), 4 TS (N=128), 5 TS128 in cluster pairs (multicast)")
+                    help="0 auto, 1 simt, 2 wgmma with 128-query blocks (dim <= 768), 3 wgmma with 64-query blocks, "
+                         "4 the same with 128-row corpus tiles, 5 = 4 in cluster pairs (multicast corpus tiles)")
     ap.add_argument("--overlap", type=int, default=1, help="1 (default): dense and BM25 routes on two streams")
     ap.add_argument("--bm25-span", type=int, default=4, help="document ranges in the first candidate launch (tuning)")
     ap.add_argument("--serial-routes", type=int, default=0,
@@ -88,10 +89,16 @@ def parse():
     ap.add_argument("--bm25-skip", type=int, default=0, help="1: candidate pass skips non-essential terms (A/B)")
     ap.add_argument("--bm25-plan", type=int, default=1, help="0: candidate CTAs resolve their posting segments themselves (A/B)")
     ap.add_argument("--dense-probe", type=int, default=0, help="measurement probe of the dense kernel (results invalid)")
-    ap.add_argument("--dense-stages", type=int, default=-1,
-                    help="cap of the dense kernel's TMA ring (0 = all smem; -1 = 3 with --overlap 1, else 0)")
+    ap.add_argument("--dense-stages", type=int, default=0,
+                    help="cap of the dense kernel's TMA ring (0 = all smem, the default: with the query block resident the "
+                         "dense CTA fills the SM's shared memory, so a cap frees no room for BM25 CTAs; 3 stages measured "
+                         "41.6 vs 31.9 ms per 10k-query launch on H100)")
     ap.add_argument("--enc-chunks", type=int, default=100_000,
                     help="chunks of the `encode` block (configs[1]: GTE-base-shaped encoder); 0 = skip the block")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the fused / sparse / dense (scores, ids, counts) of the last timed "
+                         "step as DIR/<route>_<field>.npy (float64; entries past a query's count set to -1 / 0; at most "
+                         "64 MB: a fixed seeded sample of query rows above that, listed in DIR/query_rows.npy)")
     ap.add_argument("--l2-flush", type=int, default=-1,
                     help="1: write a 512 MB buffer between steps and time each step on its own (default for <= 512 queries)")
     return ap.parse_args()
@@ -329,6 +336,32 @@ def fused_digest(fused) -> str:
     return h.hexdigest()
 
 
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, routes) -> None:
+    """Writes (scores, ids, counts) of the fused / sparse / dense lists as float64 .npy files; list entries past a
+    query's count are set to id -1 and score 0 so that two runs compare element for element.  All query rows are
+    written while the files stay within 64 MB in all; above that, a fixed seeded sample of rows (sorted).
+    ``query_rows.npy`` holds the query index of every written row."""
+    torch.cuda.synchronize()
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    nq = int(routes[0].ids.shape[0])
+    row_bytes = 8 * (1 + sum(2 * int(t.ids.shape[1]) + 1 for t in routes))     # float64 values per query row
+    keep = min(nq, (DUMP_CAP_BYTES - 4096) // row_bytes)            # 4 KB for the ten .npy headers
+    rows = np.arange(nq) if keep == nq else np.sort(np.random.default_rng(SEED).choice(nq, keep, replace=False))
+    np.save(d / "query_rows.npy", rows.astype(np.float64))
+    sel = torch.from_numpy(rows)
+    for name, t in zip(("fused", "sparse", "dense"), routes):
+        counts = t.counts.cpu()[sel].numpy().astype(np.int64)
+        ids, sc = t.ids.cpu()[sel].numpy(), t.scores.cpu()[sel].numpy()
+        valid = np.arange(ids.shape[1])[None, :] < counts[:, None]
+        np.save(d / f"{name}_ids.npy", np.where(valid, ids, -1).astype(np.float64))
+        np.save(d / f"{name}_scores.npy", np.where(valid, sc.astype(np.float64), 0.0))
+        np.save(d / f"{name}_counts.npy", counts.astype(np.float64))
+
+
 def digest_key(args) -> str:
     return f"rows={args.rows},dim={args.dim},vocab={args.vocab},queries={args.queries},k={args.k},seed={SEED}"
 
@@ -374,7 +407,7 @@ def run_ours(args):
     small_batch = args.queries <= 512
     overlap = bool(args.overlap)
     serial_routes = bool(args.serial_routes) and overlap and bool(args.pipeline)
-    stage_cap = args.dense_stages if args.dense_stages >= 0 else (3 if overlap and not small_batch and not serial_routes else 0)
+    stage_cap = args.dense_stages
     l2_flush = bool(args.l2_flush) if args.l2_flush >= 0 else small_batch
     _lib.check(L.ezr_dense_set_kernel(args.dense_kernel))
     _lib.check(L.ezr_dense_set_stage_cap(stage_cap))
@@ -413,10 +446,16 @@ def run_ours(args):
     pipelined = bool(args.pipeline) and overlap
     top = sharded if sharded is not None else ranker
 
+    last_step = {}          # (fused, sparse, dense) of the most recent step_device(): what --dump-outputs writes
+
     def step_device():
         if pipelined:
-            return top.submit(d_qvec, d_ptr, d_terms, k=k, k_out=k)
-        return hybrid(ranker, sharded, d_qvec, d_ptr, d_terms)[0]
+            t = top.submit(d_qvec, d_ptr, d_terms, k=k, k_out=k)
+            last_step["out"] = (t.fused, t.sparse, t.dense)
+            return t
+        out = hybrid(ranker, sharded, d_qvec, d_ptr, d_terms)
+        last_step["out"] = out
+        return out[0]
 
     def step_cal():
         return hybrid(ranker_seq, sharded_seq, d_qvec, d_ptr, d_terms)[0]
@@ -505,6 +544,8 @@ def run_ours(args):
     ms, per_step = timed(step_device, args.steps, drain=top.join)
     sampler.end()
     launches_timed = L.ezr_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_step["out"])      # before later submits reuse the result buffers
     prof_timed = read_prof()
     _lib.check(L.ezr_profile_enable(0))
     last = hybrid(ranker, sharded, d_qvec, d_ptr, d_terms)      # results of the measured configuration, all queries
@@ -580,14 +621,14 @@ def run_ours(args):
     pk_file = ROOT / "MEASURED_PEAKS.json"
     if pk_file.exists():
         peaks = json.loads(pk_file.read_text())
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet 3350 GB/s"
     long_step = ms > 2000.0          # a seconds-long loop settles at the sustained clock
     tf_key = "bf16_tflops_sustained" if long_step else "bf16_tflops"
-    tf_peak = float(peaks.get(tf_key, 1590.0 if not long_step else 1400.0))
+    tf_peak = float(peaks.get(tf_key, 989.0))                   # H100 SXM data sheet, dense bf16
     tf_src = (f"measured (MEASURED_PEAKS.json {tf_key}: "
               + ("kernel timed inside a seconds-long loop)" if long_step else "burst figure, the timed loop lasts well under 2 s)")
-              if tf_key in peaks else "fallback")
+              if tf_key in peaks else "H100 SXM data sheet 989 TFLOP/s")
     dense_flops = 2.0 * n_rows_local * args.dim * args.queries          # per launch: every query x every local row
     kernels = {}
     two_phase = prof["bm25_cand"][1] > 0
@@ -607,20 +648,17 @@ def run_ours(args):
         kernels["dense_tc"]["TFLOPs"] = dense_flops / (kernels["dense_tc"]["avg_ms"] * 1e-3) / 1e12
         kernels["dense_tc"]["queries_per_corpus_pass"] = min(args.queries, 128)
     dom = max(kernels, key=lambda n_: kernels[n_]["avg_ms"]) if kernels else None
-    traffic = None
-    tfile = ROOT / "profiles" / "traffic.json"
-    if tfile.exists() and dom:
-        traffic = json.loads(tfile.read_text()).get(dom if not small_batch else dom + "_b64")
     timing_note = (f"per-kernel durations: CUDA events on the launch stream over {max(args.cal_steps, 1)} calibration "
                    f"steps with the two routes back to back on one stream (same kernels, same launch shapes as the "
                    f"timed region); avg_ms_in_timed_region = the same events over the {args.steps} timed steps"
                    + (", where the routes share the SMs" if overlap else ""))
     roofline = None
-    # SURVEY.md 8(d): the dense scan is HBM-bound while queries per corpus pass stay below the ridge (~220)
-    dense_hbm_bound = args.queries <= 220
+    # SURVEY.md 8(d): the dense scan is HBM-bound while queries per corpus pass stay below the H100 ridge
+    # (989 TFLOP/s / 3.35 TB/s, about 295 flop/byte)
+    dense_hbm_bound = args.queries <= 295
     if dom == "dense_tc" and not dense_hbm_bound:
         roofline = {"bound": "tensor", "kernel": dom, "achieved": kernels[dom]["TFLOPs"], "peak": tf_peak,
-                    "unit": "TFLOP/s", "frac": kernels[dom]["TFLOPs"] / tf_peak, "traffic": traffic,
+                    "unit": "TFLOP/s", "frac": kernels[dom]["TFLOPs"] / tf_peak,
                     "peak_source": tf_src, "timing": timing_note, "kernels": kernels}
     elif dom:
         note = {"dense_tc": "algorithmic bytes = one pass over the corpus shard (N_s x D x 2) + queries + outputs "
@@ -628,7 +666,7 @@ def run_ours(args):
                 "bm25_cand": "algorithmic bytes = postings touched (4 B packed word each) + candidate ids",
                 "bm25_score": "algorithmic bytes = postings touched (12 B each) + outputs"}[dom]
         roofline = {"bound": "hbm", "kernel": dom, "achieved": kernels[dom]["GBps"], "peak": hbm_peak, "unit": "GB/s",
-                    "frac": kernels[dom]["GBps"] / hbm_peak, "traffic": traffic, "peak_source": peak_src,
+                    "frac": kernels[dom]["GBps"] / hbm_peak, "peak_source": peak_src,
                     "timing": timing_note, "kernels": kernels, "note": note}
     if roofline:
         roofline["other_kernels"] = others
@@ -683,7 +721,7 @@ def run_ours(args):
                    "steps_pipelined": pipelined, "routes_serial_on_side_stream": serial_routes,
                    "dense_ring_stages_cap": stage_cap, "timed_region_starts_from": "query vectors + term ids",
                    "l2": ("explicit flush: 512 MB written between steps, every step timed on its own" if l2_flush else
-                          "inputs larger than L2 (corpus shard and postings >> 126 MB), no explicit flush"),
+                          "inputs larger than L2 (corpus shard and postings >> 50 MB), no explicit flush"),
                    "parallelism": f"rows{world}"},
         "e2e": {"value": e2e_v, "unit": "queries/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "ms_per_step": ms_e2e / args.steps,

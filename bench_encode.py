@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Encoder-side measurement for BASELINE.json configs[1]: "GTE-base 768-d encode + cosine top-10, 100k chunks,
-1k queries, 1xB200" (SURVEY.md 8(d): tensor-bound; report TFLOP/s vs the measured bf16 peak).
+1k queries" on one H100 (SURVEY.md 8(d): tensor-bound; report TFLOP/s vs the measured bf16 peak).
 
     python bench_encode.py [--arch bert|qwen2] [--chunks N] [--batch 512]         # one JSON line
     python bench.py --workload encode                                              # the same block as the bench line
@@ -136,7 +136,7 @@ def encode_block(dev, arch: str = "bert", chunks: int = 100_000, queries: int = 
         peaks = json.loads(pk.read_text())
     long_run = ms_corpus > 2000.0
     key = "bf16_tflops_sustained" if long_run else "bf16_tflops"
-    peak = float(peaks.get(key, 1400.0 if long_run else 1590.0))
+    peak = float(peaks.get(key, 989.0))                  # H100 SXM data sheet, dense bf16
     gemm_ms, attn_ms = prof["enc_gemm"][0], prof["enc_attn"][0]
     gemm_tf = (flops_local - attn_flops_local) / (gemm_ms * 1e-3) / 1e12 if gemm_ms else None
     attn_tf = attn_flops_local / (attn_ms * 1e-3) / 1e12 if attn_ms else None
@@ -158,7 +158,7 @@ def encode_block(dev, arch: str = "bert", chunks: int = 100_000, queries: int = 
         "other_ms": prof["enc_other"][0], "gpu_launches": int(launches),
         "queries": {"n": queries, "encode_plus_top10_ms": ms_query, "queries_per_s": queries / (ms_query * 1e-3),
                     "corpus_rows_searched": index.n_rows},
-        "peak_tflops": peak, "peak_source": f"MEASURED_PEAKS.json {key}" if key in peaks else "fallback",
+        "peak_tflops": peak, "peak_source": f"MEASURED_PEAKS.json {key}" if key in peaks else "H100 SXM data sheet",
         "timing": "CUDA events around the whole corpus encode (max over ranks); per-kernel sums from ezr_profile_* events",
         "corpus_rows_written_in_place": True, "dtype": "bf16", "data": "synthetic ids, random-init weights",
         "parity": parity,

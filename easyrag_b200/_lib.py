@@ -155,7 +155,7 @@ def require_cuda() -> None:
     """Product paths call this: there is no CPU implementation to fall back to."""
     import torch
     if not torch.cuda.is_available():
-        raise EzrError("easyrag_b200 needs a CUDA device (sm_100a); no CPU fallback exists")
+        raise EzrError("easyrag_b200 needs a CUDA device (sm_90a); no CPU fallback exists")
     check(lib().ezr_device_check(), "ezr_device_check")
 
 

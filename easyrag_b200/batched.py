@@ -177,6 +177,7 @@ def rrf_fuse(ids_a: torch.Tensor, cnt_a: torch.Tensor, ids_b: torch.Tensor, cnt_
     """HybridRetriever.reciprocal_rank_fusion (retrievers.py:256-274) for a batch; list a = sparse, b = dense."""
     L = _lib.lib()
     dev = ids_a.device
+    canon = _device_canon(canon, dev)
     assert ids_a.shape == ids_b.shape and ids_a.dtype == torch.int32 and ids_b.dtype == torch.int32
     nq, stride = ids_a.shape
     if out is None:
@@ -189,11 +190,17 @@ def rrf_fuse(ids_a: torch.Tensor, cnt_a: torch.Tensor, ids_b: torch.Tensor, cnt_
     return out
 
 
+def _device_canon(canon: Optional[torch.Tensor], dev) -> Optional[torch.Tensor]:
+    """The kernels read ``canon`` on the device: a host tensor is copied over (a host address is not valid there)."""
+    return None if canon is None else canon.to(device=dev, dtype=torch.int32).contiguous()
+
+
 def fusion_simple(ids_a: torch.Tensor, sc_a: torch.Tensor, cnt_a: torch.Tensor, ids_b: torch.Tensor, sc_b: torch.Tensor,
                   cnt_b: torch.Tensor, k_out: int, canon: Optional[torch.Tensor] = None, stream=None) -> TopK:
     """HybridRetriever.fusion (retrievers.py:239-253) for a batch."""
     L = _lib.lib()
     dev = ids_a.device
+    canon = _device_canon(canon, dev)
     nq, stride = ids_a.shape
     sa = sc_a.to(torch.float64).contiguous()
     sb = sc_b.to(torch.float64).contiguous()
@@ -216,6 +223,7 @@ def fuse_lists(ids: Sequence[torch.Tensor], counts: Sequence[torch.Tensor], k_ou
     L = _lib.lib()
     n = len(ids)
     dev = ids[0].device
+    canon = _device_canon(canon, dev)
     nq, width = ids[0].shape
     ids = [t.contiguous() for t in ids]
     assert all(t.shape == (nq, width) and t.dtype == torch.int32 for t in ids) and len(counts) == n

@@ -1,4 +1,4 @@
-"""Builds the CUDA extension in-tree: easyrag_b200/_lib/libeasyrag_b200.so (sm_100a only).
+"""Builds the CUDA extension in-tree: easyrag_b200/_lib/libeasyrag_b200.so (sm_90a only).
 
 ``python -m easyrag_b200.build`` or ``__graft_entry__.build()``.  nvcc cross-compiles
 without a GPU; the .so is git-ignored but travels to the GPU box with the tree.
@@ -18,7 +18,7 @@ LIB = OUT_DIR / "libeasyrag_b200.so"
 STAMP = OUT_DIR / "build.stamp"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--cudart", "static",
@@ -75,7 +75,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         raise RuntimeError("nvcc failed; see easyrag_b200/_lib/build.log")
     if verbose:
         print("\n".join(log))
-    link = [nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "--cudart", "static",
+    link = [nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "--cudart", "static",
             "-Xcompiler", "-fPIC", "-o", str(LIB), *objs]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

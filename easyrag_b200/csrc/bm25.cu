@@ -76,10 +76,9 @@ __global__ void bm25_range_index_kernel(const int64_t* __restrict__ indptr, cons
 }
 
 // ---------------------------------------------------------------- scoring --
-// Launch shapes, swept on B200 (profiles/README.md).  The ordered kernel alone preferred (range, threads, CTAs/SM) =
-// (4096, 256, 6) at 19.6 ms per 10k queries over (8192, 512, 3) at 21.3 ms; since the two-phase path
-// (bm25_pk.cuh) took over the fused top-k, the range is chosen for ITS candidate pass, which is issue bound and
-// wants fewer, larger CTAs: (8192 docs, 256 threads, 6 CTAs/SM, 8 loads in flight) 6.9 ms vs (4096, 256, 8, 4) 7.9 ms.
+// Launch shapes.  Since the two-phase path (bm25_pk.cuh) took over the fused top-k, the range is chosen for ITS
+// candidate pass, which is issue bound and wants fewer, larger CTAs (8192 documents, 256 threads, 6 CTAs/SM).  These
+// shapes were chosen on an earlier GPU generation and have not been re-swept on the H100.
 #ifndef EZR_BM25_RANGE
 #define EZR_BM25_RANGE 8192
 #endif
@@ -94,7 +93,7 @@ constexpr int kBmThreads = EZR_BM25_THREADS;
 constexpr int kBmGroup = kBmThreads / 32;    // lanes per group: 32 group maxima bound the k-th score (k <= 32)
 static_assert(kBmGroup == 8 || kBmGroup == 16 || kBmGroup == 32, "BM25 CTA must have 256, 512 or 1024 threads");
 constexpr int kBmMaxT = 12;      // query terms preloaded per round (queries are 4-12 terms; longer ones loop)
-constexpr int kBmRpc = 1;        // document ranges per CTA (1: measured faster than 4 on B200, see DESIGN.md)
+constexpr int kBmRpc = 1;        // document ranges per CTA
 
 struct Bm25Params {
     const int64_t* indptr;
@@ -625,9 +624,9 @@ static int bm25_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int
 
 
 // ---- two-phase path (bm25_pk.cuh) ----
-// ezr_bm25_set_skipping.  OFF by default: measured on the 1M x 10k-query step the candidate pass drops from 7.7 to
-// 6.6 ms but the rescoring grows from 0.28 to 2.3 ms (profiles/r02i_*), because candidates then only carry partial
-// lower bounds and the running bound tightens more slowly.  Kept (and parity-tested) as the starting point for a
+// ezr_bm25_set_skipping.  OFF by default: the candidate pass reads fewer postings but the rescoring grows, because
+// candidates then only carry partial lower bounds and the running bound tightens more slowly (not re-measured on
+// the H100).  Kept (and parity-tested) as the starting point for a
 // version that refines the bounds between chunks.
 static int g_bm25_skip = 0;
 static int g_bm25_span = 4;     // ezr_bm25_set_span: ranges in the first candidate launch (then the same again, then doubling)

@@ -27,9 +27,9 @@
 // bound B exists, bm25_bound_kernel marks as NON-ESSENTIAL the tokens with the smallest gm whose sum NE stays
 // below kPkNeNum/kPkNeDen of B - 1.  The candidate pass does not read their postings at all: with
 // Q = Q_ess + Q_ne and Q_ne <= NE, a document with Q >= B - 1 has Q_ess >= B - 1 - NE, so that becomes the
-// crossing threshold.  The high-df terms have the smallest weights and the longest lists.  Round 1 pushed those
-// relaxed crossers as candidates with partial bounds (L = Q_ess, U = L + NE): the candidate pass got 14% faster but
-// candidates multiplied and the rescoring ate the gain (profiles/r02i_*).  Round 2 COMPLETES the relaxed crossers
+// crossing threshold.  The high-df terms have the smallest weights and the longest lists.  Pushing those relaxed
+// crossers as candidates with partial bounds (L = Q_ess, U = L + NE) made the candidate pass faster, but candidates
+// multiplied and the rescoring ate the gain.  So the kernel COMPLETES the relaxed crossers
 // inside the candidate kernel (binary search of each skipped token's postings for just those documents) and then
 // applies the exact test, so the candidate set and the bounds are those of a full pass (L = U = Q).
 #pragma once
@@ -135,8 +135,7 @@ __global__ void bm25_term_max_kernel(const int64_t* __restrict__ indptr, const u
 // ---- per (query, range, token): where the token's postings of that range start and how many there are ----
 // Resolved ONCE per candidate launch by fully parallel threads (token -> term -> range table -> offsets is a chain of
 // three dependent loads); bm25_cand_kernel then starts from one coalesced 8-byte load per lane instead of walking that
-// chain inside every (query, range) CTA while seven of its eight warps wait at a barrier (ncu, round 2: 55% of the
-// candidate pass's warp samples sat at barriers).
+// chain inside every (query, range) CTA while seven of its eight warps wait at a barrier.
 __global__ void bm25_plan_kernel(const Bm25Params p, int r_begin, int n_r, int n_queries, int2* __restrict__ plan) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (int64_t)n_queries * n_r * kPkPlanTok) return;

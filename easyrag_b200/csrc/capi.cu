@@ -22,8 +22,8 @@ int sm_count() {
     static int cached = 0;
     if (cached) return cached;
     int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
     cached = n;
     return n;
 }
@@ -101,8 +101,8 @@ int ezr_device_check(void) {
     EZR_CUDA(cudaGetDevice(&dev));
     EZR_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
     EZR_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-    if (major != 10) {
-        ezr::set_error("easyrag_b200 is built for sm_100a only; device %d is sm_%d%d", dev, major, minor);
+    if (major != 9 || minor != 0) {
+        ezr::set_error("easyrag_b200 is built for sm_90a only; device %d is sm_%d%d", dev, major, minor);
         return EZR_ERR_ARCH;
     }
     return EZR_OK;

@@ -2,7 +2,7 @@
 //
 // Replaces QdrantRetriever._aretrieve's vector search (retrievers.py:37-52 ->
 // QdrantVectorStore.aquery on a Distance.COSINE collection, ingestion.py:180-182).
-// The fast path is the tcgen05/TMEM kernel in dense_tc.cu (bf16, dim % 64 == 0,
+// The fast path is the wgmma kernel in dense_tc.cu (bf16, dim % 64 == 0, dim <= 1024,
 // k <= 16); everything else (odd dims, k up to 1024 as used by the drop-in
 // retrievers with f_topk_1 = 288) goes through the kernel below: a plain tiled
 // fp32-FMA score kernel writing a block of score rows, followed by the generic
@@ -113,7 +113,6 @@ static int simt_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64
 }
 
 static thread_local int g_force_kernel = 0;
-static const int g_default_variant = 2;   // auto: persistent TS kernel (queries in TMEM), 128-row corpus tiles
 static thread_local const char* g_last_kernel = "none";
 
 }  // namespace ezr
@@ -146,8 +145,8 @@ extern "C" {
 
 int ezr_dense_set_kernel(int32_t which) {
     EZR_CHECK_ARG(which >= 0 && which <= 5,
-                  "dense_set_kernel: 0 auto, 1 simt, 2 tcgen05 (SS), 3 tcgen05 (TS, N=64), 4 tcgen05 (TS, N=128), "
-                  "5 tcgen05 (TS, N=128, cluster pairs with multicast corpus tiles)");
+                  "dense_set_kernel: 0 auto, 1 simt, 2 wgmma (128-query blocks, dim <= 768), 3 wgmma (64-query blocks), "
+                  "4 wgmma (64-query blocks, 128-row corpus tiles), 5 = 4 in cluster pairs (multicast corpus tiles)");
     g_force_kernel = which;
     return EZR_OK;
 }
@@ -193,25 +192,19 @@ int ezr_dense_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t
     const __nv_bfloat16* q = reinterpret_cast<const __nv_bfloat16*>(queries_bf16);
     const bool tc_ok = dense_tc_supported(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k);
     if (g_force_kernel >= 2 && !tc_ok) {
-        set_error("dense_topk: tcgen05 kernel forced but shape unsupported (dim=%d k=%d ld=%lld)", dim, k,
+        set_error("dense_topk: wgmma kernel forced but shape unsupported (dim=%d k=%d ld=%lld)", dim, k,
                   (long long)ld_corpus);
         return EZR_ERR_UNSUPPORTED;
     }
     if (tc_ok && g_force_kernel != 1) {
-        // 0 = SS, 1 = TS with 64-row tiles, 2 = TS with 128-row tiles, 3 = TS128 in cluster pairs (multicast corpus tiles)
-        int variant = g_force_kernel == 5 ? 3 : g_force_kernel == 4 ? 2 : g_force_kernel == 3 ? 1
-                      : (g_force_kernel == 2 ? 0 : g_default_variant);
-        // auto: with the whole shared memory for the ring and enough query blocks to pair up, the cluster-pair form
-        // (each corpus tile pulled from L2 once per pair) measured 10% faster (10.2 vs 11.2 ms per 10k-query launch,
-        // profiles/R2e_bench_k5_seq.json); with a capped ring (routes overlapped) the two forms measured the same
-        if (g_force_kernel == 0 && g_dense_stage_cap == 0 && n_queries >= 8 * 128) variant = 3;
-        if (dim > 768 && variant == 0) {
-            set_error("dense_topk: the SS tcgen05 kernel supports dim <= 768 (got %d)", dim);
-            return EZR_ERR_UNSUPPORTED;
-        }
-        g_last_kernel = variant == 3 ? "tcgen05-ts128-mc2" : variant == 2 ? "tcgen05-ts128" : variant == 1 ? "tcgen05-ts" : "tcgen05";
+        // auto (measured on one H100, 1M rows): 128-query blocks while they fit (dim <= 768) and the batch fills them
+        // (31.9 vs 34.9 ms for 10k queries at dim 768); otherwise 64-query blocks with 128-row corpus tiles
+        // (dim 1024, 10k queries: 43.6 vs 60.4 ms for 64-row tiles; 64 queries at dim 768: 0.59 vs 0.68 ms)
+        const bool wide_block = dense_tc_max_qw(dim) == 2 && n_queries > 64;
+        const int form = g_force_kernel >= 2 ? g_force_kernel - 2 : (wide_block ? 0 : 2);
+        g_last_kernel = dense_tc_form_name(form);
         return dense_tc_topk(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k, doc_group, q_group, id_base,
-                             out_scores, out_ids, out_counts, workspace, workspace_bytes, st, variant);
+                             out_scores, out_ids, out_counts, workspace, workspace_bytes, st, form);
     }
     g_last_kernel = "simt";
     return simt_topk(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k, doc_group, q_group, id_base, out_scores,

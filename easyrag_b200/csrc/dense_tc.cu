@@ -1,18 +1,18 @@
-// Dense cosine top-k on 5th-gen tensor cores: TMA -> shared memory -> tcgen05.mma -> TMEM,
-// with the top-k taken in the epilogue straight from the accumulators.
+// Dense cosine top-k on the Hopper tensor cores: TMA -> shared memory -> wgmma -> registers, with the top-k taken
+// in the epilogue straight from the accumulators.
 //
 // Replaces the vector search behind QdrantRetriever._aretrieve (retrievers.py:37-52;
 // Distance.COSINE, ingestion.py:180-182).  Work decomposition (DESIGN.md "Dense"):
-//   grid = (corpus slices, query blocks).  A CTA keeps one block of 128 queries resident in
-//   shared memory for its whole life (A operand, K-major, 128B-swizzled, dim/64 chunks of
-//   16 KB) and streams its slice of corpus rows through a ring of 8 KB TMA stages
-//   (B operand: 64 rows x 64 bf16).  One elected thread issues tcgen05.mma 128x64x16 into one
-//   of four 64-column TMEM accumulator stages; the four epilogue warps read a finished stage
-//   with tcgen05.ld (one query row per thread) and push the 64 scores through a per-thread
-//   register-resident sorted list of k <= 16.  Scores never reach HBM: per (query, slice) the
-//   CTA writes k (score,id) pairs, and a warp-per-query merge produces the final list.
-// The corpus is read from HBM exactly once per query block, so a launch is HBM-bound for
-// blocks of <= ~220 queries (ridge of measured bf16 peak / measured HBM bandwidth).
+//   persistent CTAs walk work units (corpus split s, query block b), ordered split-major: a CTA keeps ONE query block
+//   for a long run of corpus rows (n_rows / n_splits), so the per-thread top-k lists warm up once per unit and almost
+//   nothing passes the threshold afterwards, and the query blocks resident at the same time stream the SAME corpus
+//   split, so a corpus tile is fetched from HBM once and served to the other CTAs from the L2.
+//   A query block (QW x 64 queries, QW = 2 consumer warpgroups for dim <= 768, 1 above) sits in shared memory for
+//   the whole unit (A operand, K-major, 128B-swizzled, 64 x 64 TMA boxes); the corpus rows stream through a ring of
+//   8 KB TMA stages (B operand: 64 rows x 64 bf16).  Each consumer warpgroup issues wgmma.m64n64k16 into 32 fp32
+//   registers per thread and scans its scores with a per-thread register-resident sorted list of k <= 16 per query
+//   row.  Scores never reach HBM: per (query, split) the four threads that share a query row write k (score, id)
+//   pairs each, and a warp-per-query merge produces the final list.
 #include "ezr_common.cuh"
 #include "ptx.cuh"
 #include "dense_tc.h"
@@ -23,29 +23,20 @@ namespace ezr {
 int g_dense_probe = 0;       // ezr_dense_set_probe
 int g_dense_stage_cap = 0;   // 0: use all shared memory for the TMA ring (ezr_dense_set_stage_cap)
 
-constexpr int TC_M = 128;       // queries per CTA = UMMA M
-constexpr int TC_N = 64;        // corpus rows per tile = UMMA N
+constexpr int TC_TN = 64;       // the narrower corpus tile (rows): bounds the number of corpus splits
 constexpr int TC_KC = 64;       // bf16 per k-chunk = one 128-byte swizzle row
-constexpr int TC_MAXD = 768;       // SS variant: whole query block in shared memory
-constexpr int TS_MAXD = 1024;      // TS variant: 768 columns in TMEM + up to 256 in shared memory
-constexpr int TS_TMEM_KC = 12;     // 64-row-tile TS kernel: k-chunks of the query block in tensor memory (12 x 32 = 384 columns;
-                                   // the 128-row-tile kernel keeps 8, see dense_ts_kernel)
-constexpr int TC_ACC = 4;       // TMEM accumulator stages (TC_N fp32 columns each)
-constexpr int TC_MAX_STAGES = 26;
-constexpr int TC_THREADS = 192; // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2-5: epilogue
+constexpr int TC_MAXD = 1024;
+constexpr int TC_LISTS = 4;     // lists per (query, split): the four threads of a query row
+constexpr int TC_MAX_STAGES = 32;
 constexpr int TC_KMAX = 16;
-constexpr int TS_ACC = 2;          // TS variant: accumulator stages
-constexpr int TS_THREADS = 320;    // TS variant: TMA warp, MMA warp, 8 epilogue warps
-constexpr int TC_A_CHUNK_BYTES = TC_M * TC_KC * 2;   // 16384
-constexpr int TC_B_STAGE_BYTES = TC_N * TC_KC * 2;   // 8192
+constexpr int TC_A_BOX_BYTES = 64 * TC_KC * 2;       // 8192: 64 queries x one k-chunk
+constexpr int TC_B_STAGE_BYTES = TC_TN * TC_KC * 2;  // 8192
 constexpr int TC_SMEM_LIMIT = 232448;                 // 227 KB opt-in maximum per CTA
 
 struct TcParams {
-    const __nv_bfloat16* queries;   // TS variant reads the query block straight from global memory
-    int64_t ldq;
     int dim;
     int64_t n_rows;
-    int rows_per_slice;   // multiple of TC_N
+    int rows_per_slice;   // multiple of the corpus tile rows
     int n_queries;
     int kchunks;          // dim / 64
     int n_stages;
@@ -53,231 +44,139 @@ struct TcParams {
     int id_base;
     const int32_t* doc_group;
     const int32_t* q_group;
-    float* part_s;        // [n_queries][n_slices][k]
+    float* part_s;        // [n_queries][n_slices][TC_LISTS][k]
     int32_t* part_id;
-    int32_t* bound;       // TS variant: [n_queries] float bits (0 = none) of a proven lower bound of each query's final
-                          // k-th best score, raised by every finished unit; later units of the query start from it
+    int32_t* bound;       // [n_queries] float bits (0 = none) of a proven lower bound of each query's final k-th best
+                          // score, raised by every finished unit; later units of the query start from it
     int n_slices;
-    int n_qblocks;        // TS variant: units = n_slices x n_qblocks, walked by persistent CTAs
-    int kps;              // TS variant: k-chunks (TMA boxes) per pipeline stage: 1, 2 or 4
-    int probe;            // measurement probes (ezr_dense_set_probe): 1 = no TMA loads, 2 = no MMAs, 3 = no epilogue scan; results are garbage
+    int n_qblocks;        // units = n_slices x n_qblocks, walked by persistent CTAs
+    int probe;            // measurement probes (ezr_dense_set_probe): 1 = no TMA loads, 2 = no MMAs, 4 = no epilogue scan; results are garbage
 };
 
 struct TcBarriers {
-    uint64_t a_full;
-    uint64_t ahi_full;     // TS variant, dim > 768: the shared-memory tail of the query block has landed (TMA)
-    uint64_t ahi_empty;    // ... and every MMA of the previous unit that read it has retired (tcgen05.commit)
+    uint64_t a_full;       // the unit's query block has landed
+    uint64_t a_empty;      // ... and every MMA of the previous unit that read it has retired (one arrival per consumer)
     uint64_t b_full[TC_MAX_STAGES];
     uint64_t b_empty[TC_MAX_STAGES];
-    uint64_t acc_full[TC_ACC];
-    uint64_t acc_empty[TC_ACC];
-    uint32_t tmem_base;
 };
 
-// KT = compile-time list length (smallest of 4/8/12/16 >= k) so the per-thread list stays in registers
-template <bool FILTER, int KT>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-dense_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
-                const TcParams p) {
-    extern __shared__ unsigned char smem_dyn[];
-    // 128B swizzle needs 1024-byte aligned tiles
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    unsigned char* smem_a = smem;
-    unsigned char* smem_b = smem + (size_t)p.kchunks * TC_A_CHUNK_BYTES;
-    TcBarriers* bars = reinterpret_cast<TcBarriers*>(smem_b + (size_t)p.n_stages * TC_B_STAGE_BYTES);
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const int slice = blockIdx.x;
-    const int q0 = blockIdx.y * TC_M;
-    const int64_t row_begin = (int64_t)slice * p.rows_per_slice;
-    const int64_t row_end = min(p.n_rows, row_begin + p.rows_per_slice);
-    const int n_tiles = (int)((row_end - row_begin + TC_N - 1) / TC_N);
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&map_q);
-        ptx::prefetch_tensormap(&map_c);
-        ptx::mbar_init(&bars->a_full, 1);
-        for (int i = 0; i < p.n_stages; ++i) {
-            ptx::mbar_init(&bars->b_full[i], 1);
-            ptx::mbar_init(&bars->b_empty[i], 1);
-        }
-        for (int i = 0; i < TC_ACC; ++i) {
-            ptx::mbar_init(&bars->acc_full[i], 1);
-            ptx::mbar_init(&bars->acc_empty[i], 4);
-        }
-        ptx::fence_barrier_init();
-    }
-    if (warp == 1) ptx::tmem_alloc<TC_ACC * TC_N>(&bars->tmem_base);
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = bars->tmem_base;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            // ---------------- TMA producer ----------------
-            ptx::mbar_expect_tx(&bars->a_full, (uint32_t)p.kchunks * TC_A_CHUNK_BYTES);
-            for (int kc = 0; kc < p.kchunks; ++kc)
-                ptx::tma_load_2d_hint(smem_a + (size_t)kc * TC_A_CHUNK_BYTES, &map_q, &bars->a_full, kc * TC_KC, q0,
-                                      ptx::kEvictLast);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = 0; t < n_tiles; ++t) {
-                const int row0 = (int)(row_begin + (int64_t)t * TC_N);
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    ptx::mbar_wait(&bars->b_empty[stage], phase ^ 1);
-                    ptx::mbar_expect_tx(&bars->b_full[stage], TC_B_STAGE_BYTES);
-                    ptx::tma_load_2d_hint(smem_b + (size_t)stage * TC_B_STAGE_BYTES, &map_c, &bars->b_full[stage],
-                                          kc * TC_KC, row0, ptx::kEvictFirst);
-                    if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ---------------- MMA issuer ----------------
-            constexpr uint32_t idesc = ptx::make_idesc_bf16(TC_M, TC_N);
-            ptx::mbar_wait(&bars->a_full, 0);
-            ptx::tc_fence_after();
-            const uint32_t a_base = ptx::smem_u32(smem_a);
-            const uint32_t b_base = ptx::smem_u32(smem_b);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = 0; t < n_tiles; ++t) {
-                const int as = t % TC_ACC;
-                const uint32_t aph = (uint32_t)(t / TC_ACC) & 1u;
-                ptx::mbar_wait(&bars->acc_empty[as], aph ^ 1);
-                ptx::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(as * TC_N);
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    ptx::mbar_wait(&bars->b_full[stage], phase);
-                    ptx::tc_fence_after();
-                    const uint32_t a_addr = a_base + (uint32_t)kc * TC_A_CHUNK_BYTES;
-                    const uint32_t b_addr = b_base + (uint32_t)stage * TC_B_STAGE_BYTES;
+// candidates arrive in increasing id order per list, so on equal score the newcomer (higher id) ranks first under the
+// canonical order: ">=" everywhere
+template <int KT>
+__device__ __forceinline__ void list_insert(float (&ts)[KT], int (&ti)[KT], float cv, int ci) {
 #pragma unroll
-                    for (int k4 = 0; k4 < TC_KC / 16; ++k4) {
-                        ptx::umma_f16_ss(d_tmem, ptx::make_desc_sw128(a_addr + k4 * 32),
-                                         ptx::make_desc_sw128(b_addr + k4 * 32), idesc, (uint32_t)((kc | k4) != 0));
-                    }
-                    ptx::umma_commit(&bars->b_empty[stage]);          // frees the smem stage when the MMAs retire
-                    if (kc == p.kchunks - 1) ptx::umma_commit(&bars->acc_full[as]);
-                    if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else {
-        // ---------------- epilogue: one query row per thread ----------------
-        const int quad = warp & 3;                 // TMEM lane quadrant this warp may access
-        const int m = quad * 32 + lane;
-        const int qg = q0 + m;
-        const bool active = qg < p.n_queries;
-        const int k = p.k;
-        int want = -1;
-        if (FILTER && active) want = p.q_group[qg];
-        float ts[KT];
-        int ti[KT];
-#pragma unroll
-        for (int j = 0; j < KT; ++j) { ts[j] = -INFINITY; ti[j] = -1; }
-        float thr = -INFINITY;
-
-        for (int t = 0; t < n_tiles; ++t) {
-            const int as = t % TC_ACC;
-            const uint32_t aph = (uint32_t)(t / TC_ACC) & 1u;
-            ptx::mbar_wait(&bars->acc_full[as], aph);
-            ptx::tc_fence_after();
-            const int64_t row0 = row_begin + (int64_t)t * TC_N;
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * TC_N);
-#pragma unroll
-            for (int half = 0; half < TC_N / 32; ++half) {
-                uint32_t r[32];
-                ptx::tmem_ld_32x32(taddr + half * 32, r);
-                ptx::tmem_ld_wait();
-                if (half == TC_N / 32 - 1) {
-                    // accumulator stage is in registers: hand it back to the MMA warp
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&bars->acc_empty[as]);
-                }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float v = __uint_as_float(r[j]) + 0.0f;       // -0.0 -> +0.0
-                    const int64_t doc = row0 + half * 32 + j;
-                    bool ok = active && doc < row_end && v >= thr;
-                    if (FILTER) {
-                        if (ok && want != -1) ok = (__ldg(p.doc_group + doc) == want);
-                    }
-                    if (ok) {
-                        // candidates arrive in increasing id order, so on equal score the newcomer (higher id)
-                        // ranks first under the canonical order: ">=" everywhere.
-                        float cv = v;
-                        int ci = (int)doc + p.id_base;
-#pragma unroll
-                        for (int s = 0; s < KT; ++s) {
-                            const bool b = cv >= ts[s];
-                            const float fs = ts[s];
-                            const int is = ti[s];
-                            ts[s] = b ? cv : fs;
-                            ti[s] = b ? ci : is;
-                            cv = b ? fs : cv;
-                            ci = b ? is : ci;
-                        }
-                        thr = ts[KT - 1];
-                    }
-                }
-            }
-        }
-        if (active) {
-            const int64_t o = ((int64_t)qg * p.n_slices + slice) * k;
-#pragma unroll
-            for (int s = 0; s < KT; ++s) {
-                if (s < k) {
-                    p.part_s[o + s] = ts[s];
-                    p.part_id[o + s] = ti[s];
-                }
-            }
-        }
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<TC_ACC * TC_N>(tmem_base);
+    for (int s = 0; s < KT; ++s) {
+        const bool b = cv >= ts[s];
+        const float fs = ts[s];
+        const int is = ti[s];
+        ts[s] = b ? cv : fs;
+        ti[s] = b ? ci : is;
+        cv = b ? fs : cv;
+        ci = b ? is : ci;
     }
 }
 
-// TS variant (default): the 128-query block lives in TENSOR MEMORY (columns [0, dim/2)); the A operand of
-// tcgen05.mma is read from TMEM, which frees ~190 KB of shared memory for the corpus ring (26 x 8 KB in flight).
-// Persistent CTAs walk work units (corpus split s, query block b), ordered split-major: a CTA keeps ONE query block
-// for a LONG run of corpus rows (n_rows / n_splits), so the per-thread top-k lists warm up once per unit and
-// almost nothing passes the threshold afterwards, and the query blocks that are resident at the same time stream
-// the SAME corpus split, so every corpus tile is fetched from HBM once and served to the other CTAs from L2.
-// TMEM (TN = 64):  A at columns [0, 384), two 64-column accumulator stages at [384, 512).
-// TMEM (TN = 128): A at columns [0, 256) (k-chunks 0..7; the rest of the query block sits in shared memory and
-// those k-steps use the SS form), two 128-column accumulator stages at [256, 512).  The TS form reads its A
-// operand from tensor memory at 64 B/clk (4 KB per 128x16 slab = 64 cycles per MMA, measured: a pipeline run
-// with the TMA loads removed still takes 64 cycles per N=64 MMA, twice its 32-cycle floor), so only N >= 128
-// keeps the tensor pipe busy: one MMA then covers 128 corpus rows in the same 64 cycles.
+// The top-k list of one query row of a thread (accumulator fragment row r + 8 H).
+template <int KT>
+struct RowList {
+    float ts[KT];
+    int ti[KT];
+    float seed, thr;
+    int qg, want;
+    bool active;
+};
+
+// this thread's TN / 4 scores of row H of a TN-row corpus tile (columns 8 j + 2 (lane % 4) + e, in increasing
+// document order)
+template <bool FILTER, int KT, int H, int TN>
+__device__ __forceinline__ void scan_row(const float (&acc)[TN / 2], RowList<KT>& L, int64_t doc0, int64_t left,
+                                         const TcParams& p) {
+    constexpr int NJ = TN / 8;
+    float mx = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) mx = fmaxf(mx, fmaxf(acc[4 * j + 2 * H], acc[4 * j + 2 * H + 1]));
+    if (p.probe & 4) mx = -INFINITY;
+    if (!(L.active && mx >= L.thr)) return;
+    // slow path: which of them reach the threshold (bit 2 j + e), then ONE copy of the insertion code over the set
+    // bits, in increasing document order
+    uint32_t mask = 0;
+    float vals[2 * NJ];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float v = acc[4 * j + 2 * H + e];
+            vals[2 * j + e] = v;
+            mask |= ((8 * j + e < left && v >= L.thr) ? 1u : 0u) << (2 * j + e);
+        }
+    }
+    while (mask) {
+        const int b = __ffs(mask) - 1;
+        mask &= mask - 1;
+        const float v = vals[b] + 0.0f;                           // -0.0 -> +0.0
+        const int64_t doc = doc0 + 8 * (b >> 1) + (b & 1);
+        bool ok = v >= L.thr;                                     // thr may have risen inside this batch
+        if (FILTER) {
+            if (ok && L.want != -1) ok = (__ldg(p.doc_group + doc) == L.want);
+        }
+        if (ok) {
+            list_insert<KT>(L.ts, L.ti, v, (int)doc + p.id_base);
+            L.thr = fmaxf(L.ts[KT - 1], L.seed);
+        }
+    }
+}
+
+template <int KT>
+__device__ __forceinline__ void row_start(RowList<KT>& L, int qg, const TcParams& p, bool filter) {
+    L.qg = qg;
+    L.active = qg < p.n_queries;
+    L.want = (filter && L.active) ? p.q_group[qg] : -1;
+#pragma unroll
+    for (int j = 0; j < KT; ++j) { L.ts[j] = -INFINITY; L.ti[j] = -1; }
+    // Seed: k documents with a score >= seed are already known for this query (published by units that finished
+    // earlier, possibly on other SMs), so nothing below it can reach the final top-k; equal scores stay in (ties are
+    // decided by id in the merge).
+    L.seed = -INFINITY;
+    if (L.active) {
+        const int b = *reinterpret_cast<const volatile int32_t*>(p.bound + qg);
+        if (b > 0) L.seed = __int_as_float(b);
+    }
+    L.thr = L.seed;
+}
+
+template <int KT>
+__device__ __forceinline__ void row_finish(const RowList<KT>& L, int slice, int list, const TcParams& p) {
+    if (!L.active) return;
+    const int k = p.k;
+    if (L.ti[k - 1] >= 0 && L.ts[k - 1] > 0.f)
+        atomicMax(p.bound + L.qg, __float_as_int(L.ts[k - 1]));   // positive floats order like their bit patterns
+    const int64_t o = (((int64_t)L.qg * p.n_slices + slice) * TC_LISTS + list) * k;
+#pragma unroll
+    for (int s = 0; s < KT; ++s) {
+        if (s < k) {
+            p.part_s[o + s] = L.ts[s];
+            p.part_id[o + s] = L.ti[s];
+        }
+    }
+}
+
+// Warpgroup 0 = TMA producer (one thread), then QW consumer warpgroups (64 query rows each; a warpgroup issuing wgmma
+// must start at a warp index that is a multiple of 4).  KT = compile-time list length (smallest of 4/8/12/16 >= k) so
+// the per-thread lists stay in registers; TN = corpus rows per tile (wgmma N, 64 or 128).
 // CL = 2: CTAs run in cluster pairs on the same corpus split with two neighbouring query blocks; each CTA loads HALF of
-// every corpus tile and TMA-multicasts it into both CTAs' rings (map_c then has boxes of TN / 2 rows), so a pair
-// pulls each tile from L2 once instead of twice.  The stage hand-over is the only other change: a ring stage is free
-// when BOTH CTAs' MMAs have released it (tcgen05.commit multicast), because the peer's multicast writes into it.
-template <bool FILTER, int KT, int TN, int CL>
-__global__ void __launch_bounds__(TS_THREADS, 1)
-dense_ts_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
-                const TcParams p) {
-    constexpr int TMEM_KC = TN == 64 ? 12 : 8;             // k-chunks of A held in tensor memory
-    constexpr int ACC_COL0 = TMEM_KC * (TC_KC / 2);        // first accumulator column
-    constexpr int B_CHUNK_BYTES = TN * TC_KC * 2;          // one k-chunk of a corpus tile
-    static_assert(ACC_COL0 + TS_ACC * TN <= 512, "tensor memory layout");
+// every corpus tile and TMA-multicasts it into both CTAs' rings, so a pair pulls each tile from L2 once instead of
+// twice.  A ring stage is then free only when the consumers of BOTH CTAs have released it (the peer's multicast writes
+// into it), so consumers arrive on the stage's empty barrier in both CTAs.
+template <bool FILTER, int KT, int QW, int TN, int CL>
+__global__ void __launch_bounds__(128 + 128 * QW, 1)
+dense_wgmma_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
+                   const TcParams p) {
+    constexpr int B_STAGE_BYTES = TN * TC_KC * 2;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    const int kc_tm = min(p.kchunks, TMEM_KC);             // k-chunks of A in tensor memory
-    const int kc_sm = p.kchunks - kc_tm;                   // k-chunks of A in shared memory (dim > 768)
-    unsigned char* smem_ahi = smem;
-    unsigned char* smem_b = smem + (size_t)kc_sm * TC_A_CHUNK_BYTES;
-    TcBarriers* bars = reinterpret_cast<TcBarriers*>(smem_b + (size_t)p.n_stages * p.kps * B_CHUNK_BYTES);
+    unsigned char* smem_a = smem;                                             // [QW][kchunks] boxes of 8 KB
+    unsigned char* smem_b = smem + (size_t)QW * p.kchunks * TC_A_BOX_BYTES;
+    TcBarriers* bars = reinterpret_cast<TcBarriers*>(smem_b + (size_t)p.n_stages * B_STAGE_BYTES);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -287,281 +186,131 @@ dense_ts_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     const int qb_groups = (p.n_qblocks + CL - 1) / CL;
     const int n_units = p.n_slices * qb_groups;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&map_c);
         ptx::prefetch_tensormap(&map_q);
-        ptx::mbar_init(&bars->a_full, 4);
-        ptx::mbar_init(&bars->ahi_full, 1);
-        ptx::mbar_init(&bars->ahi_empty, 1);
+        ptx::mbar_init(&bars->a_full, 1);
+        ptx::mbar_init(&bars->a_empty, QW);
         for (int i = 0; i < p.n_stages; ++i) {
             ptx::mbar_init(&bars->b_full[i], 1);
-            ptx::mbar_init(&bars->b_empty[i], CL);
-        }
-        for (int i = 0; i < TS_ACC; ++i) {
-            ptx::mbar_init(&bars->acc_full[i], 1);
-            ptx::mbar_init(&bars->acc_empty[i], 8);
+            ptx::mbar_init(&bars->b_empty[i], QW * CL);
         }
         ptx::fence_barrier_init();
     }
-    if (warp == 1) ptx::tmem_alloc<512>(&bars->tmem_base);
-    ptx::tc_fence_before();
     __syncthreads();
     if (CL > 1) ptx::cluster_sync();     // the peer's barriers exist before anything is multicast into this CTA
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = bars->tmem_base;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            // ---------------- TMA producer: corpus tiles of every unit of this CTA, back to back ----------------
+    if (warp < 4) {
+        ptx::regs_dealloc<40>();
+        if (threadIdx.x == 0) {
+            // ---------------- TMA producer: query block + corpus tiles of every unit of this CTA, back to back
             int stage = 0;
             uint32_t phase = 0;
             int ui = 0;
             for (int u = worker; u < n_units; u += n_workers, ++ui) {
                 const int slice = u / qb_groups;
+                const int q0 = ((u % qb_groups) * CL + rank) * (64 * QW);
                 const int64_t row_begin = (int64_t)slice * p.rows_per_slice;
                 const int64_t row_end = min(p.n_rows, row_begin + p.rows_per_slice);
                 const int n_tiles = (int)((row_end - row_begin + TN - 1) / TN);
-                if (kc_sm > 0) {
-                    // tail of the query block (columns >= 768) -> shared memory, once the previous unit's MMAs are done
-                    const int q0 = ((u % qb_groups) * CL + rank) * TC_M;
-                    ptx::mbar_wait(&bars->ahi_empty, ((uint32_t)ui & 1u) ^ 1u);
-                    ptx::mbar_expect_tx(&bars->ahi_full, (uint32_t)kc_sm * TC_A_CHUNK_BYTES);
-                    for (int j = 0; j < kc_sm; ++j)
-                        ptx::tma_load_2d(smem_ahi + (size_t)j * TC_A_CHUNK_BYTES, &map_q, &bars->ahi_full,
-                                         (kc_tm + j) * TC_KC, q0);
-                }
+                ptx::mbar_wait(&bars->a_empty, ((uint32_t)ui & 1u) ^ 1u);    // the previous unit's MMAs are done
+                ptx::mbar_expect_tx(&bars->a_full, (uint32_t)(QW * p.kchunks * TC_A_BOX_BYTES));
+                for (int w = 0; w < QW; ++w)
+                    for (int kc = 0; kc < p.kchunks; ++kc)
+                        ptx::tma_load_2d_hint(smem_a + (size_t)(w * p.kchunks + kc) * TC_A_BOX_BYTES, &map_q, &bars->a_full,
+                                              kc * TC_KC, q0 + w * 64, ptx::kEvictLast);
                 for (int t = 0; t < n_tiles; ++t) {
                     const int row0 = (int)(row_begin + (int64_t)t * TN);
-                    for (int kc = 0; kc < p.kchunks; kc += p.kps) {
+                    for (int kc = 0; kc < p.kchunks; ++kc) {
                         ptx::mbar_wait(&bars->b_empty[stage], phase ^ 1);
-                        if ((p.probe & 1)) {                       // probe: pipeline without the loads
+                        unsigned char* dst = smem_b + (size_t)stage * B_STAGE_BYTES;
+                        if (p.probe & 1) {                       // probe: pipeline without the loads
                             ptx::mbar_arrive(&bars->b_full[stage]);
-                            if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-                            continue;
-                        }
-                        ptx::mbar_expect_tx(&bars->b_full[stage], (uint32_t)(p.kps * B_CHUNK_BYTES));
-                        unsigned char* dst = smem_b + (size_t)stage * (size_t)(p.kps * B_CHUNK_BYTES);
-                        for (int j = 0; j < p.kps; ++j) {
-                            if (CL == 1)
-                                ptx::tma_load_2d(dst + (size_t)j * B_CHUNK_BYTES, &map_c, &bars->b_full[stage],
-                                                 (kc + j) * TC_KC, row0);
-                            else     // this CTA's rows [rank * TN / 2, +TN / 2) of the tile, into both CTAs
-                                ptx::tma_load_2d_mcast(dst + (size_t)j * B_CHUNK_BYTES + (size_t)rank * (B_CHUNK_BYTES / CL),
-                                                       &map_c, &bars->b_full[stage], (kc + j) * TC_KC,
-                                                       row0 + rank * (TN / CL), (uint16_t)0x3);
+                        } else if (CL == 1) {
+                            ptx::mbar_expect_tx(&bars->b_full[stage], B_STAGE_BYTES);
+                            // no evict_first hint: the CTAs on the same split find this tile in L2 (measured faster)
+                            ptx::tma_load_2d(dst, &map_c, &bars->b_full[stage], kc * TC_KC, row0);
+                        } else {
+                            // the whole tile lands here (both halves); this CTA's half goes to both CTAs
+                            ptx::mbar_expect_tx(&bars->b_full[stage], B_STAGE_BYTES);
+                            ptx::tma_load_2d_mcast(dst + (size_t)rank * (B_STAGE_BYTES / CL), &map_c, &bars->b_full[stage],
+                                                   kc * TC_KC, row0 + rank * (TN / CL), (uint16_t)((1u << CL) - 1u));
                         }
                         if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer ----------------
-        // The whole warp walks the loop (warp-uniform control flow, so descriptor arithmetic stays on the uniform
-        // datapath); only the tcgen05 instructions themselves are issued by one elected lane.
-        constexpr uint32_t idesc = ptx::make_idesc_bf16(TC_M, TN);
-        const uint64_t b_desc0 = ptx::make_desc_sw128(ptx::smem_u32(smem_b));
-        const uint64_t ahi_desc0 = ptx::make_desc_sw128(ptx::smem_u32(smem_ahi));
+    } else {
+        // ---------------- consumers: warpgroup cw owns query rows [64 cw, 64 cw + 64) of the block
+        ptx::regs_alloc<QW == 2 ? 232 : 240>();
+        const int cw = (threadIdx.x >> 7) - 1;
+        const int wq = warp & 3;                            // warp within the warpgroup
+        const bool leader = (threadIdx.x & 127) == 0;
+        const uint32_t a_base = ptx::smem_u32(smem_a) + (uint32_t)(cw * p.kchunks * TC_A_BOX_BYTES);
+        const uint32_t b_base = ptx::smem_u32(smem_b);
+        // hand a ring stage back: to this CTA's producer, and with CL = 2 to the peer's (whose multicast fills it too)
+        auto release = [&](int s) {
+            if (CL == 1) ptx::mbar_arrive(&bars->b_empty[s]);
+            else
+                for (int c = 0; c < CL; ++c) ptx::mbar_arrive_cluster(&bars->b_empty[s], (uint32_t)c);
+        };
         int stage = 0;
         uint32_t phase = 0;
-        int it = 0;           // tiles issued by this CTA so far (accumulator stage / phase)
-        int ui = 0;           // units started (phase of a_full / ahi_full)
+        int ui = 0;
         for (int u = worker; u < n_units; u += n_workers, ++ui) {
             const int slice = u / qb_groups;
+            const int q0 = ((u % qb_groups) * CL + rank) * (64 * QW) + cw * 64;
             const int64_t row_begin = (int64_t)slice * p.rows_per_slice;
             const int64_t row_end = min(p.n_rows, row_begin + p.rows_per_slice);
             const int n_tiles = (int)((row_end - row_begin + TN - 1) / TN);
-            ptx::mbar_wait(&bars->a_full, (uint32_t)ui & 1u);      // this unit's query block is in TMEM
-            if (kc_sm > 0) ptx::mbar_wait(&bars->ahi_full, (uint32_t)ui & 1u);   // ... and its tail in shared memory
-            ptx::tc_fence_after();
-            for (int t = 0; t < n_tiles; ++t, ++it) {
-                const int as = it % TS_ACC;
-                const uint32_t aph = (uint32_t)(it / TS_ACC) & 1u;
-                ptx::mbar_wait(&bars->acc_empty[as], aph ^ 1);
-                ptx::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(ACC_COL0 + as * TN);
-                for (int kc = 0; kc < p.kchunks; kc += p.kps) {
+            // this thread's two query rows (accumulator fragment rows r and r + 8)
+            RowList<KT> L0, L1;
+            row_start<KT>(L0, q0 + wq * 16 + (lane >> 2), p, FILTER);
+            row_start<KT>(L1, q0 + wq * 16 + (lane >> 2) + 8, p, FILTER);
+            ptx::mbar_wait(&bars->a_full, (uint32_t)ui & 1u);
+
+            for (int t = 0; t < n_tiles; ++t) {
+                float acc[TN / 2];
+#pragma unroll
+                for (int i = 0; i < TN / 2; ++i) acc[i] = 0.f;
+                int prev = -1;
+                for (int kc = 0; kc < p.kchunks; ++kc) {
                     ptx::mbar_wait(&bars->b_full[stage], phase);
-                    ptx::tc_fence_after();
-                    const uint32_t a_tmem = tmem_base + (uint32_t)(kc * (TC_KC / 2));
-                    const uint64_t b_desc = b_desc0 + (uint64_t)(stage * p.kps * (B_CHUNK_BYTES >> 4));
-                    if (ptx::elect_one()) {
-                        const int nj = (p.probe & 2) ? (kc == 0 ? 1 : 0) : p.kps;     // probe 2: one k-chunk per tile
+                    if (!(p.probe & 2) || kc == 0) {
+                        ptx::wgmma_fence();
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {                                 // kps <= 4: static offsets
-                            if (j < nj) {
-                                if (kc + j < kc_tm) {
-#pragma unroll
-                                    for (int k4 = 0; k4 < TC_KC / 16; ++k4)
-                                        ptx::umma_f16_ts(d_tmem, a_tmem + j * (TC_KC / 2) + k4 * 8,
-                                                         b_desc + (uint64_t)(j * (B_CHUNK_BYTES >> 4) + k4 * 2), idesc,
-                                                         (uint32_t)((kc | j | k4) != 0));
-                                } else {
-                                    const uint64_t a_desc =
-                                        ahi_desc0 + (uint64_t)((kc + j - kc_tm) * (TC_A_CHUNK_BYTES >> 4));
-#pragma unroll
-                                    for (int k4 = 0; k4 < TC_KC / 16; ++k4)
-                                        ptx::umma_f16_ss(d_tmem, a_desc + (uint64_t)(k4 * 2),
-                                                         b_desc + (uint64_t)(j * (B_CHUNK_BYTES >> 4) + k4 * 2), idesc,
-                                                         1u);
-                                }
-                            }
+                        for (int k4 = 0; k4 < TC_KC / 16; ++k4) {
+                            const uint64_t da = ptx::make_desc_sw128(a_base + (uint32_t)(kc * TC_A_BOX_BYTES + k4 * 32));
+                            const uint64_t db = ptx::make_desc_sw128(b_base + (uint32_t)(stage * B_STAGE_BYTES + k4 * 32));
+                            if constexpr (TN == 64) ptx::wgmma_ss_n64(acc, da, db, (uint32_t)((kc | k4) != 0));
+                            else ptx::wgmma_ss_n128(acc, da, db, (uint32_t)((kc | k4) != 0));
                         }
-                        if (CL == 1) ptx::umma_commit(&bars->b_empty[stage]);
-                        else ptx::umma_commit_mcast(&bars->b_empty[stage], (uint16_t)0x3);   // frees the stage in both CTAs
-                        if (kc + p.kps >= p.kchunks) {
-                            ptx::umma_commit(&bars->acc_full[as]);
-                            if (kc_sm > 0 && t == n_tiles - 1) ptx::umma_commit(&bars->ahi_empty);   // unit done with A_hi
-                        }
+                        ptx::wgmma_commit();
                     }
-                    __syncwarp();
+                    // the previous chunk's MMAs are done: hand its stage back to the producer(s)
+                    ptx::wgmma_wait<1>();
+                    if (prev >= 0 && leader) release(prev);
+                    prev = stage;
                     if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
                 }
-            }
-        }
-    } else {
-        // ---------------- epilogue: 8 warps, two per TMEM lane quadrant ----------------
-        // Thread (quad, lane) owns query row quad*32+lane; the two warps of a quadrant split every 64-row corpus tile
-        // into rows [0,32) and [32,64) and each keeps its own sorted list, so a query ends a unit with two lists
-        // (both go to the merge).  The first four warps also stage the query block into tensor memory.
-        const int quad = warp & 3;
-        const int half = (warp - 2) >> 2;          // 0: tile rows 0..31, 1: tile rows 32..63
-        const int m = quad * 32 + lane;
-        const int k = p.k;
-        int it = 0;
-        for (int u = worker; u < n_units; u += n_workers) {
-            const int slice = u / qb_groups;
-            const int q0 = ((u % qb_groups) * CL + rank) * TC_M;
-            const int64_t row_begin = (int64_t)slice * p.rows_per_slice;
-            const int64_t row_end = min(p.n_rows, row_begin + p.rows_per_slice);
-            const int n_tiles = (int)((row_end - row_begin + TN - 1) / TN);
-            const int qg = q0 + m;
-            const bool active = qg < p.n_queries;
-            int want = -1;
-            if (FILTER && active) want = p.q_group[qg];
-            // All MMAs of the previous unit have retired (its last acc_full was waited on below), so the A
-            // columns may be overwritten: 64 bf16 (= 32 packed 32-bit columns) per tcgen05.st.
-            if (half == 0) {
-                const uint4* src = reinterpret_cast<const uint4*>(p.queries + (int64_t)(active ? qg : 0) * p.ldq);
-                for (int kc = 0; kc < kc_tm; ++kc) {
-                    uint32_t r[32];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-                        if (active) v = __ldg(src + kc * 8 + j);
-                        r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
-                    }
-                    ptx::tmem_st_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(kc * (TC_KC / 2)), r);
+                ptx::wgmma_wait<0>();
+                ptx::fence_regs(acc);
+                if (leader) {
+                    release(prev);
+                    if (t == n_tiles - 1) ptx::mbar_arrive(&bars->a_empty);    // the unit's last read of the query block
                 }
-                ptx::tmem_st_wait();
-                ptx::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&bars->a_full);
+                // ---- epilogue: this thread's TN / 4 scores of each of its two rows
+                const int64_t doc0 = row_begin + (int64_t)t * TN + (lane & 3) * 2;
+                scan_row<FILTER, KT, 0, TN>(acc, L0, doc0, row_end - doc0, p);
+                scan_row<FILTER, KT, 1, TN>(acc, L1, doc0, row_end - doc0, p);
             }
-            float ts[KT];
-            int ti[KT];
-#pragma unroll
-            for (int j = 0; j < KT; ++j) { ts[j] = -INFINITY; ti[j] = -1; }
-            // Seed: k documents with a score >= seed are already known for this query (published by units that
-            // finished earlier, possibly on other SMs), so nothing below it can reach the final top-k; equal scores
-            // stay in (ties are decided by id in the merge).  Without a seed the list warms up from -inf in every unit.
-            float seed = -INFINITY;
-            if (active) {
-                const int b = *reinterpret_cast<const volatile int32_t*>(p.bound + qg);
-                if (b > 0) seed = __int_as_float(b);
-            }
-            float thr = seed;
-
-            for (int t = 0; t < n_tiles; ++t, ++it) {
-                const int as = it % TS_ACC;
-                const uint32_t aph = (uint32_t)(it / TS_ACC) & 1u;
-                ptx::mbar_wait(&bars->acc_full[as], aph);
-                ptx::tc_fence_after();
-                constexpr int SUBS = TN / 64;            // 32-column batches per epilogue warp and tile
-#pragma unroll 1
-                for (int sub = 0; sub < SUBS; ++sub) {
-                const int64_t doc0 = row_begin + (int64_t)t * TN + half * (TN / 2) + sub * 32;
-                uint32_t r[32];
-                ptx::tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) +
-                                       (uint32_t)(ACC_COL0 + as * TN + half * (TN / 2) + sub * 32), r);
-                ptx::tmem_ld_wait();
-                if (sub == SUBS - 1) {
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&bars->acc_empty[as]);   // scores are in registers: stage is free
-                }
-                // Fast path (straight-line, static register indices): the maximum of the 32 scores.  After the
-                // lists have warmed up most batches of 32 end here.
-                float mx = -INFINITY;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(r[j]));
-                if (p.probe & 4) mx = -INFINITY;
-                if (active && mx >= thr) {
-                    // Slow path: which of the 32 reach the threshold (bit mask, static indices), then ONE copy of the
-                    // insertion code over the set bits, in increasing document order (a fully unrolled version is
-                    // ~100 KB of SASS and thrashes the instruction cache).
-                    float tmp[32];
-                    uint32_t mask = 0;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float v = __uint_as_float(r[j]);
-                        tmp[j] = v;
-                        mask |= (v >= thr ? 1u : 0u) << j;
-                    }
-                    const int64_t left = row_end - doc0;                      // rows of this batch inside the unit
-                    if (left < 32) mask &= (left <= 0) ? 0u : ((1u << (int)left) - 1u);
-                    while (mask) {
-                        const int j = __ffs(mask) - 1;
-                        mask &= mask - 1;
-                        const float v = tmp[j] + 0.0f;                        // -0.0 -> +0.0
-                        const int64_t doc = doc0 + j;
-                        bool ok = v >= thr;                                   // thr may have risen inside this batch
-                        if (FILTER) {
-                            if (ok && want != -1) ok = (__ldg(p.doc_group + doc) == want);
-                        }
-                        if (ok) {
-                            // candidates arrive in increasing id order, so on equal score the newcomer (higher id)
-                            // ranks first under the canonical order: ">=" everywhere.
-                            float cv = v;
-                            int ci = (int)doc + p.id_base;
-#pragma unroll
-                            for (int s = 0; s < KT; ++s) {
-                                const bool b = cv >= ts[s];
-                                const float fs = ts[s];
-                                const int is = ti[s];
-                                ts[s] = b ? cv : fs;
-                                ti[s] = b ? ci : is;
-                                cv = b ? fs : cv;
-                                ci = b ? is : ci;
-                            }
-                            thr = fmaxf(ts[KT - 1], seed);
-                        }
-                    }
-                }
-                }   // sub
-            }
-            if (active && ti[k - 1] >= 0 && ts[k - 1] > 0.f)
-                atomicMax(p.bound + qg, __float_as_int(ts[k - 1]));      // positive floats order like their bit patterns
-            if (active) {
-                const int64_t o = (((int64_t)qg * p.n_slices + slice) * 2 + half) * k;
-#pragma unroll
-                for (int s = 0; s < KT; ++s) {
-                    if (s < k) {
-                        p.part_s[o + s] = ts[s];
-                        p.part_id[o + s] = ti[s];
-                    }
-                }
-            }
+            row_finish<KT>(L0, slice, lane & 3, p);
+            row_finish<KT>(L1, slice, lane & 3, p);
         }
     }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (CL > 1) ptx::cluster_sync();     // no CTA leaves while its peer may still multicast into it / arrive on its barriers
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<512>(tmem_base);
-    }
+    // no CTA leaves while its peer may still multicast into it or arrive on its barriers
+    if (CL > 1) ptx::cluster_sync();
 }
 
 // ------------------------------------------------------------------ host ----
@@ -599,18 +348,12 @@ int encode_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t cols, uint6
     return EZR_OK;
 }
 
-static int tc_slices(int64_t n_rows) {
-    const int64_t tiles = (n_rows + TC_N - 1) / TC_N;
-    const int sms = sm_count();
-    return (int)(tiles < sms ? tiles : sms);
-}
-
-static int tc_rows_per_slice(int64_t n_rows, int slices, int tn = TC_N) {
+static int tc_rows_per_slice(int64_t n_rows, int slices, int tn) {
     const int64_t tiles = (n_rows + tn - 1) / tn;
     return (int)((tiles + slices - 1) / slices) * tn;
 }
 
-// TS variant: number of corpus splits.  Units = splits x query blocks are walked by `sms` persistent CTAs.
+// Number of corpus splits.  Units = splits x query blocks are walked by `sms` persistent CTAs.
 // Cost model: makespan = waves x (unit length + re-warm time of the per-thread top-k lists), in units of the time
 // one CTA needs to stream the whole corpus (~45 GB/s per SM); re-warming costs ~20 us per unit.
 static int ts_choose_splits(int qblocks, int64_t n_rows, int dim, int sms, int tn) {
@@ -633,7 +376,7 @@ static int ts_choose_splits(int qblocks, int64_t n_rows, int dim, int sms, int t
 
 bool dense_tc_supported(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
                         int n_queries, int64_t ldq, int k) {
-    if (dim % TC_KC != 0 || dim > TS_MAXD || dim <= 0) return false;
+    if (dim % TC_KC != 0 || dim > TC_MAXD || dim <= 0) return false;
     if (k < 1 || k > TC_KMAX) return false;
     if (ldc % 8 != 0 || ldq % 8 != 0) return false;
     if ((reinterpret_cast<uintptr_t>(corpus) & 15) || (reinterpret_cast<uintptr_t>(queries) & 15)) return false;
@@ -642,35 +385,48 @@ bool dense_tc_supported(const __nv_bfloat16* corpus, int64_t n_rows, int dim, in
 }
 
 size_t dense_tc_workspace(int64_t n_rows, int dim, int n_queries, int k) {
-    if (dim % TC_KC != 0 || dim > TS_MAXD || k > TC_KMAX || n_rows < 1) return 0;
-    const int slices = tc_slices(n_rows);
-    const size_t n = (size_t)n_queries * slices * k * 2;      // TS variant: two lists per (query, split)
+    if (dim % TC_KC != 0 || dim > TC_MAXD || k > TC_KMAX || n_rows < 1) return 0;
+    const int64_t tiles = (n_rows + TC_TN - 1) / TC_TN;
+    const int slices = (int)(tiles < sm_count() ? tiles : sm_count());     // upper bound of ts_choose_splits
+    const size_t n = (size_t)n_queries * slices * k * TC_LISTS;
     return align_up(n * 4, 256) * 2 + align_up((size_t)n_queries * 4, 256);      // + the per-query score bounds
 }
+
+int dense_tc_max_qw(int dim) { return dim <= 768 ? 2 : 1; }
+
+// kernel forms: (query blocks of 64 * QW rows, corpus tiles of TN rows, CTAs per cluster)
+struct TcForm { int qw, tn, cl; const char* name; };
+static const TcForm kForms[4] = {{2, 64, 1, "wgmma"}, {1, 64, 1, "wgmma-q64"}, {1, 128, 1, "wgmma-q64-n128"},
+                                 {1, 128, 2, "wgmma-q64-n128-mc2"}};
+
+const char* dense_tc_form_name(int form) { return kForms[form].name; }
 
 int dense_tc_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
                   int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
                   float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
-                  cudaStream_t st, int variant) {
+                  cudaStream_t st, int form) {
     const size_t need = dense_tc_workspace(n_rows, dim, n_queries, k);
     if (ws_bytes < need || !ws) {
-        set_error("dense_topk(tcgen05): workspace %zu < %zu", ws_bytes, need);
+        set_error("dense_topk(wgmma): workspace %zu < %zu", ws_bytes, need);
         return EZR_ERR_WORKSPACE;
     }
+    if (form < 0 || form > 3) {
+        set_error("dense_topk(wgmma): bad kernel form %d", form);
+        return EZR_ERR_INVALID;
+    }
+    const TcForm f = kForms[form];
+    if (f.qw > dense_tc_max_qw(dim)) {
+        set_error("dense_topk(wgmma): %d-query blocks need dim <= 768 (got %d)", 64 * f.qw, dim);
+        return EZR_ERR_UNSUPPORTED;
+    }
     TcParams p;
-    p.queries = queries;
-    p.ldq = ldq;
     p.dim = dim;
     p.n_rows = n_rows;
-    p.n_qblocks = (n_queries + TC_M - 1) / TC_M;
-    const bool ts = variant >= 1;
-    const int cl = variant == 3 ? 2 : 1;                        // variant 3: TS128 in cluster pairs (multicast corpus tiles)
-    if (variant == 3) variant = 2;
-    const int tn = variant == 2 ? 128 : TC_N;                   // corpus rows per tile (UMMA N)
-    const int tmem_kc = variant == 2 ? 8 : TS_TMEM_KC;          // k-chunks of the query block in tensor memory
-    const int qb_groups = (p.n_qblocks + cl - 1) / cl;          // work units per corpus split
-    p.n_slices = ts ? ts_choose_splits(qb_groups, n_rows, dim, sm_count() / cl, tn) : tc_slices(n_rows);
-    p.rows_per_slice = tc_rows_per_slice(n_rows, p.n_slices, tn);
+    p.n_qblocks = (n_queries + 64 * f.qw - 1) / (64 * f.qw);
+    const int sms = sm_count();
+    const int qb_groups = (p.n_qblocks + f.cl - 1) / f.cl;     // work units per corpus split
+    p.n_slices = ts_choose_splits(qb_groups, n_rows, dim, sms / f.cl, f.tn);
+    p.rows_per_slice = tc_rows_per_slice(n_rows, p.n_slices, f.tn);
     // with the rounded-up slice size the last slices may be empty: shrink to the non-empty ones
     p.n_slices = (int)((n_rows + p.rows_per_slice - 1) / p.rows_per_slice);
     p.n_queries = n_queries;
@@ -679,97 +435,73 @@ int dense_tc_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t 
     p.id_base = id_base;
     p.doc_group = doc_group;
     p.q_group = q_group;
-    if (!ts && dim > TC_MAXD) {
-        set_error("dense_topk(tcgen05 SS): dim=%d > %d; use the TS variant", dim, TC_MAXD);
-        return EZR_ERR_UNSUPPORTED;
-    }
-    const int kc_sm = p.kchunks > tmem_kc ? p.kchunks - tmem_kc : 0;
-    const size_t a_bytes = ts ? (size_t)kc_sm * TC_A_CHUNK_BYTES : (size_t)p.kchunks * TC_A_CHUNK_BYTES;
-    const size_t chunk_bytes = (size_t)tn * TC_KC * 2;          // one k-chunk of a corpus tile
-    const size_t fixed = 1024 /*alignment slack*/ + sizeof(TcBarriers) + 64;
     p.probe = g_dense_probe;
-    p.kps = 1;
-    if (variant == 1) p.kps = (p.kchunks % 4 == 0) ? 4 : ((p.kchunks % 2 == 0) ? 2 : 1);
-    if (variant == 2) p.kps = (p.kchunks % 2 == 0) ? 2 : 1;     // 32 KB per stage either way
-    int stages = (int)((TC_SMEM_LIMIT - fixed - a_bytes) / ((size_t)p.kps * chunk_bytes));
+    const size_t a_bytes = (size_t)f.qw * p.kchunks * TC_A_BOX_BYTES;
+    const size_t b_stage = (size_t)f.tn * TC_KC * 2;
+    const size_t fixed = 1024 /*alignment slack*/ + sizeof(TcBarriers);
+    int stages = (int)((TC_SMEM_LIMIT - fixed - a_bytes) / b_stage);
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
     // leave shared memory to kernels of another stream (the BM25 route) when the caller overlaps the two routes
     if (g_dense_stage_cap > 0 && stages > g_dense_stage_cap) stages = g_dense_stage_cap;
     if (stages < 2) {
-        set_error("dense_topk(tcgen05): dim=%d leaves no room for a TMA ring", dim);
+        set_error("dense_topk(wgmma): dim=%d leaves no room for a TMA ring", dim);
         return EZR_ERR_UNSUPPORTED;
     }
     p.n_stages = stages;
-    const size_t smem = fixed + a_bytes + (size_t)stages * p.kps * chunk_bytes;
-    const int lists = ts ? 2 : 1;
-    const size_t n_part = (size_t)n_queries * p.n_slices * k * lists;
+    const size_t smem = fixed + a_bytes + (size_t)stages * b_stage;
+    const size_t n_part = (size_t)n_queries * p.n_slices * k * TC_LISTS;
     p.part_s = reinterpret_cast<float*>(ws);
     p.part_id = reinterpret_cast<int32_t*>((char*)ws + align_up(n_part * 4, 256));
     p.bound = reinterpret_cast<int32_t*>((char*)ws + need - align_up((size_t)n_queries * 4, 256));
-    if (ts) EZR_CUDA(cudaMemsetAsync(p.bound, 0, (size_t)n_queries * 4, st));
+    EZR_CUDA(cudaMemsetAsync(p.bound, 0, (size_t)n_queries * 4, st));
 
     CUtensorMap map_q, map_c;
-    int rc = encode_tmap_2d_bf16(&map_q, queries, (uint64_t)dim, (uint64_t)n_queries, (uint64_t)ldq, TC_KC, TC_M);
+    int rc = encode_tmap_2d_bf16(&map_q, queries, (uint64_t)dim, (uint64_t)n_queries, (uint64_t)ldq, TC_KC, 64);
     if (rc) return rc;
-    rc = encode_tmap_2d_bf16(&map_c, corpus, (uint64_t)dim, (uint64_t)n_rows, (uint64_t)ldc, TC_KC, (uint32_t)(tn / cl));
+    rc = encode_tmap_2d_bf16(&map_c, corpus, (uint64_t)dim, (uint64_t)n_rows, (uint64_t)ldc, TC_KC,
+                             (uint32_t)(f.tn / f.cl));
     if (rc) return rc;
 
-    const bool filter = (q_group != nullptr);
+    const int fi = (q_group != nullptr) ? 1 : 0;
     typedef void (*kern_t)(const CUtensorMap, const CUtensorMap, const TcParams);
-    static const kern_t table[4][2][4] = {
-        {{dense_tc_kernel<false, 4>, dense_tc_kernel<false, 8>, dense_tc_kernel<false, 12>, dense_tc_kernel<false, 16>},
-         {dense_tc_kernel<true, 4>, dense_tc_kernel<true, 8>, dense_tc_kernel<true, 12>, dense_tc_kernel<true, 16>}},
-        {{dense_ts_kernel<false, 4, 64, 1>, dense_ts_kernel<false, 8, 64, 1>, dense_ts_kernel<false, 12, 64, 1>,
-          dense_ts_kernel<false, 16, 64, 1>},
-         {dense_ts_kernel<true, 4, 64, 1>, dense_ts_kernel<true, 8, 64, 1>, dense_ts_kernel<true, 12, 64, 1>,
-          dense_ts_kernel<true, 16, 64, 1>}},
-        {{dense_ts_kernel<false, 4, 128, 1>, dense_ts_kernel<false, 8, 128, 1>, dense_ts_kernel<false, 12, 128, 1>,
-          dense_ts_kernel<false, 16, 128, 1>},
-         {dense_ts_kernel<true, 4, 128, 1>, dense_ts_kernel<true, 8, 128, 1>, dense_ts_kernel<true, 12, 128, 1>,
-          dense_ts_kernel<true, 16, 128, 1>}},
-        {{dense_ts_kernel<false, 4, 128, 2>, dense_ts_kernel<false, 8, 128, 2>, dense_ts_kernel<false, 12, 128, 2>,
-          dense_ts_kernel<false, 16, 128, 2>},
-         {dense_ts_kernel<true, 4, 128, 2>, dense_ts_kernel<true, 8, 128, 2>, dense_ts_kernel<true, 12, 128, 2>,
-          dense_ts_kernel<true, 16, 128, 2>}}};
+#define EZR_DENSE_FORM(QW, TN, CL)                                                                                  \
+    {{dense_wgmma_kernel<false, 4, QW, TN, CL>, dense_wgmma_kernel<false, 8, QW, TN, CL>,                           \
+      dense_wgmma_kernel<false, 12, QW, TN, CL>, dense_wgmma_kernel<false, 16, QW, TN, CL>},                        \
+     {dense_wgmma_kernel<true, 4, QW, TN, CL>, dense_wgmma_kernel<true, 8, QW, TN, CL>,                             \
+      dense_wgmma_kernel<true, 12, QW, TN, CL>, dense_wgmma_kernel<true, 16, QW, TN, CL>}}
+    static const kern_t table[4][2][4] = {EZR_DENSE_FORM(2, 64, 1), EZR_DENSE_FORM(1, 64, 1), EZR_DENSE_FORM(1, 128, 1),
+                                          EZR_DENSE_FORM(1, 128, 2)};
+#undef EZR_DENSE_FORM
     const int kt = (k + 3) / 4 - 1;
-    const int vi = cl == 2 ? 3 : variant;
-    kern_t kern = table[vi][filter ? 1 : 0][kt];
+    kern_t kern = table[form][fi][kt];
     static bool attr_done[4][2][4] = {};
-    if (!attr_done[vi][filter ? 1 : 0][kt]) {
+    if (!attr_done[form][fi][kt]) {
         EZR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
         // always configure the SM for the largest shared-memory carveout: with a capped ring the rest of the
         // shared memory is then available to co-resident CTAs of other streams
         EZR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        attr_done[vi][filter ? 1 : 0][kt] = true;
+        attr_done[form][fi][kt] = true;
     }
-    dim3 grid(p.n_slices, p.n_qblocks);
-    if (ts) {
-        const int units = p.n_slices * qb_groups;
-        const int workers = units < sm_count() / cl ? units : sm_count() / cl;
-        grid = dim3(workers * cl, 1);
-    }
+    const int units = p.n_slices * qb_groups;
+    const int workers = units < sms / f.cl ? units : sms / f.cl;
     {
         ProfScope prof(EZR_PROF_DENSE_TC, st);
-        if (cl == 1) {
-            kern<<<grid, ts ? TS_THREADS : TC_THREADS, smem, st>>>(map_q, map_c, p);
-        } else {
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = grid;
-            cfg.blockDim = dim3(TS_THREADS);
-            cfg.dynamicSmemBytes = smem;
-            cfg.stream = st;
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeClusterDimension;
-            attr[0].val.clusterDim.x = 2;
-            attr[0].val.clusterDim.y = 1;
-            attr[0].val.clusterDim.z = 1;
-            cfg.attrs = attr;
-            cfg.numAttrs = 1;
-            EZR_CUDA(cudaLaunchKernelEx(&cfg, kern, map_q, map_c, p));
-        }
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)(workers * f.cl));
+        cfg.blockDim = dim3((unsigned)(128 + 128 * f.qw));
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = (unsigned)f.cl;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        EZR_CUDA(cudaLaunchKernelEx(&cfg, kern, map_q, map_c, p));
     }
     EZR_LAUNCH_CHECK();
-    const int n_cand = p.n_slices * k * lists;
+    const int n_cand = p.n_slices * k * TC_LISTS;
     return ezr_merge_topk(p.part_s, p.part_id, EZR_F32, n_queries, n_cand, n_cand, k, out_scores, out_ids, out_counts,
                           nullptr, 0, st);
 }

@@ -1,4 +1,4 @@
-// tcgen05/TMEM dense cosine top-k (dense_tc.cu): host-side entry points.
+// wgmma dense cosine top-k (dense_tc.cu): host-side entry points.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -13,7 +13,10 @@ size_t dense_tc_workspace(int64_t n_rows, int dim, int n_queries, int k);
 int dense_tc_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
                   int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
                   float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
-                  cudaStream_t st, int variant);   // variant 0: queries in shared memory (SS), 1: in TMEM (TS)
+                  cudaStream_t st, int form);   // form 0: 128-query blocks (dim <= 768), 1: 64-query blocks,
+                                                // 2: 64-query blocks and 128-row corpus tiles, 3: 2 in cluster pairs
+const char* dense_tc_form_name(int form);
+int dense_tc_max_qw(int dim);   // 2 while the 128-query block fits shared memory beside the ring (dim <= 768), else 1
 
 extern int g_dense_probe;       // see ezr_dense_set_probe
 extern int g_dense_stage_cap;   // see ezr_dense_set_stage_cap

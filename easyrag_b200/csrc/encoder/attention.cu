@@ -7,7 +7,7 @@
 // Flash-style: one CTA = 64 query rows of one (sequence, head); K/V streamed in 64-key tiles through
 // XOR-swizzled shared memory; S = QK^T and O += PV on warp-level bf16 MMA (m16n8k16, fp32 accumulate), online
 // softmax in fp32 (exp2 with the 1/sqrt(d) scale folded in).  Attention is ~10% of the encoder FLOPs at
-// L <= 512 (SURVEY.md 8(d)); the projections around it run on tcgen05 (gemm_tc.cu).
+// L <= 512 (SURVEY.md 8(d)); the projections around it run on wgmma (gemm_tc.cu).
 #include "../ezr_common.cuh"
 
 namespace ezr {
@@ -198,7 +198,7 @@ attn_bidir_kernel(const __nv_bfloat16* __restrict__ qkv, int64_t ld, const int32
 }  // namespace ezr
 
 // The first attention kernel of this library (warp-level mma.sync), kept as an independent implementation the
-// tcgen05 kernel (attention_tc.cu) is cross-checked against: ezr_attn_set_kernel(1).
+// wgmma kernel (attention_tc.cu) is cross-checked against: ezr_attn_set_kernel(1).
 namespace ezr {
 int attn_bidir_legacy(const void* qkv, int64_t ld, const int32_t* cu_seqlens, int32_t n_seq, int32_t max_len,
                       int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, float softmax_scale, void* out, int64_t ldo,

@@ -1,62 +1,37 @@
-// Bidirectional (non-causal) multi-head attention over PACKED variable-length sequences on tcgen05 / TMEM.
+// Bidirectional (non-causal) multi-head attention over PACKED variable-length sequences on wgmma (Hopper warpgroup MMA).
 //
 // Reference: Qwen2 attention run with is_causal=False (modeling_qwen.py:289-308 eager / :704-712 SDPA, padding
 // handled by an additive mask :1037-1040) and BERT self-attention behind SentenceTransformer.encode
 // (hf_embeddings.py:118-123).  Sequences are packed, so the mask reduces to "keys beyond this sequence".
 //
 // Work item = 128 query rows of one (sequence, head).  A small plan kernel lists the (sequence, query block) pairs
-// that exist; PERSISTENT CTAs (two per SM: 256 TMEM columns and <= 96 KB of shared memory each) walk the items
-// round-robin, query blocks of one (sequence, head) next to each other so that concurrently running CTAs share its
-// K / V tiles through L2.  Barriers, tensor memory and the tensor-map prefetch are set up once per CTA, and the TMA
-// producer runs ahead into the next item.
-//   warp 0      TMA producer: Q tile per item, K / V tiles of 64 keys (one packed [tokens, (H + 2 KV) hd] matrix serves
-//               Q, K and V through two tensor maps -- 128-row and 64-row boxes; 128B swizzle; rows past the matrix are
-//               zero-filled)
-//   warp 1      tcgen05.mma issuer:  S = Q K^T   (SS form, both operands K-major in shared memory, N = keys of the tile)
-//                                    O += P V    (TS form: P is read from TENSOR MEMORY, V is the MN-major B operand
-//                                                 straight from its row-major TMA tile -- no transpose anywhere)
-//               S is DOUBLE BUFFERED: S_{j+1} = Q K_{j+1}^T is issued before the probabilities of tile j are waited for,
-//               so the softmax warps never wait for a QK^T and the tensor pipe works under the softmax.
-//   warps 2-5   softmax: one warp per TMEM lane quadrant, a thread owns one query row and all 64 key columns of a
-//               tile, read ONCE from tensor memory into registers: row max, exp2 with the 1/sqrt(d) scale folded in,
-//               probabilities written back as packed bf16 over the S columns they came from (tcgen05.st), running sum
-//               in fp32; at the end of an item O / sum -> bf16 -> global.  No cross-warp exchange anywhere.
-// The kernel is bound by the softmax arithmetic (one MUFU.EX2 per score: 16 per clock and SM), not by the tensor
-// pipe: ncu, profiles/README.md round 2.
-// TMEM columns: [0,64) / [64,128) the two S buffers (fp32), each aliased by its P (bf16 pairs, 32 columns),
-// [128, 128+hd) O.  The running maximum is lazy: O is rescaled in tensor memory (tcgen05.ld / multiply / tcgen05.st)
-// only when a row's maximum grows by more than 2^8; otherwise the stale maximum stays (p <= 256 is harmless in
-// bf16 / fp32) -- the final division by the row sum makes both choices the same function.
+// that exist; PERSISTENT CTAs walk the items round-robin, query blocks of one (sequence, head) next to each other so
+// that concurrently running CTAs share its K / V tiles through L2.
+//   warpgroup 0    TMA producer (one thread): Q tile per item, K / V tiles of 64 keys (one packed [tokens, (H + 2 KV) hd] matrix
+//                  serves Q, K and V through two tensor maps -- 128-row and 64-row boxes; 128B swizzle; rows past the
+//                  matrix are zero-filled), running ahead across items
+//   warpgroups 1-2 64 query rows each:  S = Q K^T      wgmma SS m64n64k16 (both operands K-major in shared memory)
+//                                       online softmax in registers (a row lives in the four threads of a quad)
+//                                       O += P V       wgmma RS m64n{hd}k16: P straight from the S registers as bf16
+//                                                      A fragments, V the MN-major B operand from its row-major TMA
+//                                                      tile -- no transpose anywhere
+//                  at the end of an item O / row sum -> bf16 -> global.
 #include "../ezr_common.cuh"
 #include "../ptx.cuh"
 
 namespace ezr {
 
-constexpr int AT_M = 128;                 // query rows per work item (UMMA M, one TMEM lane each)
-constexpr int AT_N = 64;                  // keys per tile (UMMA N of S = Q K^T)
-constexpr int AT_THREADS = 192;           // TMA warp, MMA warp, 4 softmax warps
+constexpr int AT_M = 128;                 // query rows per work item
+constexpr int AT_N = 64;                  // keys per tile
+constexpr int AT_THREADS = 384;           // producer warpgroup + two consumer warpgroups (wgmma needs 4-warp-aligned groups)
 constexpr int AT_BOX_BYTES = 128 * 64 * 2;   // one Q TMA box: 128 rows x 64 bf16
 constexpr int AT_KV_BOX_BYTES = AT_N * 64 * 2;   // one K / V TMA box: 64 rows x 64 bf16
-constexpr int AT_TMEM_COLS = 256;
-constexpr int AT_O_COL = 128;
-constexpr float AT_RESCALE_LOG2 = 8.0f;   // rescale O only when the row maximum grows by more than 2^8
+constexpr int AT_STAGES = 2;              // K and V rings (own barriers each)
 
-constexpr int AT_MAX_STAGES = 4;
 struct AttnBarriers {
-    uint64_t q_full[2], q_empty[2];
-    uint64_t k_full[AT_MAX_STAGES], k_empty[AT_MAX_STAGES], v_full[AT_MAX_STAGES], v_empty[AT_MAX_STAGES];
-    uint64_t s_full[2], p_full[2], o_full;
-    uint32_t tmem_base;
+    uint64_t q_full, q_empty;
+    uint64_t k_full[AT_STAGES], k_empty[AT_STAGES], v_full[AT_STAGES], v_empty[AT_STAGES];
 };
-// shared-memory shape: one Q buffer and 2-deep K / V rings (48 KB at hd 64, two CTAs per SM).  With EZR_ATTN_DEEP=1, hd 64
-// gets two Q buffers + 4-deep rings (96 KB) and the first QK^T of the NEXT work item is issued under the softmax of this
-// item's last tile -- measured on one box (session 20): 414-417 vs 416-418 TFLOP/s at L = 512, 290 vs 295 on ragged
-// batches: the two CTAs per SM already cover the item boundaries, so the switch is off.
-#ifndef EZR_ATTN_DEEP
-#define EZR_ATTN_DEEP 0          // tuning switch (variant builds): 1 = at hd 64 two Q buffers + 4-deep rings (see below); measured equal
-#endif
-__host__ __device__ constexpr int at_qbuf(int hd) { return (EZR_ATTN_DEEP && hd == 64) ? 2 : 1; }
-__host__ __device__ constexpr int at_stages(int hd) { return (EZR_ATTN_DEEP && hd == 64) ? 4 : 2; }
 
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
@@ -98,57 +73,51 @@ attn_plan_kernel(const int32_t* __restrict__ cu, int n_seq, int4* __restrict__ p
     if (tid == 0) plan_n[0] = s_base;
 }
 
+__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
+    __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&v);
+}
+
 template <int HD>
-__global__ void __launch_bounds__(AT_THREADS, 2)
-attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
-               const int4* __restrict__ plan, const int32_t* __restrict__ plan_n,
-               int n_heads, int n_kv_heads, float scale_log2, __nv_bfloat16* __restrict__ out, int64_t ldo) {
+__global__ void __launch_bounds__(AT_THREADS, 1)
+attn_wgmma_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
+                  const int4* __restrict__ plan, const int32_t* __restrict__ plan_n,
+                  int n_heads, int n_kv_heads, float scale_log2, __nv_bfloat16* __restrict__ out, int64_t ldo) {
     constexpr int CH = HD / 64;                          // 64-column TMA boxes per tile
     constexpr int Q_BYTES = CH * AT_BOX_BYTES;           // one Q tile
     constexpr int KV_BYTES = CH * AT_KV_BOX_BYTES;       // one K / V tile
-    constexpr int STAGES = at_stages(HD);                // K and V rings (own barriers each)
-    constexpr int QBUF = at_qbuf(HD);
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     unsigned char* smem_q = smem;
-    unsigned char* smem_k = smem_q + QBUF * Q_BYTES;
-    unsigned char* smem_v = smem_k + STAGES * KV_BYTES;
-    AttnBarriers* bars = reinterpret_cast<AttnBarriers*>(smem_v + STAGES * KV_BYTES);
+    unsigned char* smem_k = smem_q + Q_BYTES;
+    unsigned char* smem_v = smem_k + AT_STAGES * KV_BYTES;
+    AttnBarriers* bars = reinterpret_cast<AttnBarriers*>(smem_v + AT_STAGES * KV_BYTES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_pairs = plan_n[0];
     const int n_work = n_pairs * n_heads;                // work w: head = w / n_pairs, pair = w % n_pairs
     const int kv_group = n_heads / n_kv_heads;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&map_q);
         ptx::prefetch_tensormap(&map_kv);
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(&bars->q_full[i], 1);
-            ptx::mbar_init(&bars->q_empty[i], 1);
-            ptx::mbar_init(&bars->s_full[i], 1);
-            ptx::mbar_init(&bars->p_full[i], 4);
-        }
-        for (int i = 0; i < STAGES; ++i) {
+        ptx::mbar_init(&bars->q_full, 1);
+        ptx::mbar_init(&bars->q_empty, 2);
+        for (int i = 0; i < AT_STAGES; ++i) {
             ptx::mbar_init(&bars->k_full[i], 1);
-            ptx::mbar_init(&bars->k_empty[i], 1);
+            ptx::mbar_init(&bars->k_empty[i], 2);
             ptx::mbar_init(&bars->v_full[i], 1);
-            ptx::mbar_init(&bars->v_empty[i], 1);
+            ptx::mbar_init(&bars->v_empty[i], 2);
         }
-        ptx::mbar_init(&bars->o_full, 1);
         ptx::fence_barrier_init();
     }
-    if (warp == 1) ptx::tmem_alloc<AT_TMEM_COLS>(&bars->tmem_base);
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = bars->tmem_base;
     // every role walks the same items w = blockIdx.x, + gridDim.x, ...; the plan entry of the NEXT item is requested at
     // the top of each iteration, so no role ever waits for it
     auto plan_at = [&](int w) { return w < n_work ? __ldg(plan + w % n_pairs) : make_int4(0, 0, 0, 0); };
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        if (threadIdx.x == 0) {
             // ---------------- TMA producer: runs ahead of the consumers, across work items ----------------
             int jt = 0;                                   // K/V tiles issued so far (ring position)
             int it = 0;                                   // items started
@@ -161,14 +130,13 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
                 const int kvh = h / kv_group;
                 const int col_q = h * HD, col_k = (n_heads + kvh) * HD, col_v = (n_heads + n_kv_heads + kvh) * HD;
                 const int n_kt = (len + AT_N - 1) / AT_N;
-                const int qb = it % QBUF;
-                ptx::mbar_wait(&bars->q_empty[qb], ((uint32_t)(it / QBUF) & 1u) ^ 1u);   // the QK^T MMAs that read this buffer are done
-                ptx::mbar_expect_tx(&bars->q_full[qb], Q_BYTES);
+                ptx::mbar_wait(&bars->q_empty, ((uint32_t)it & 1u) ^ 1u);   // the QK^T MMAs that read the Q buffer are done
+                ptx::mbar_expect_tx(&bars->q_full, Q_BYTES);
                 for (int c = 0; c < CH; ++c)
-                    ptx::tma_load_2d(smem_q + qb * Q_BYTES + c * AT_BOX_BYTES, &map_q, &bars->q_full[qb], col_q + c * 64, lo + q0);
+                    ptx::tma_load_2d(smem_q + c * AT_BOX_BYTES, &map_q, &bars->q_full, col_q + c * 64, lo + q0);
                 for (int j = 0; j < n_kt; ++j, ++jt) {
-                    const int s = jt % STAGES;
-                    const uint32_t ph = (uint32_t)(jt / STAGES) & 1u;
+                    const int s = jt % AT_STAGES;
+                    const uint32_t ph = (uint32_t)(jt / AT_STAGES) & 1u;
                     const int row = lo + j * AT_N;
                     ptx::mbar_wait(&bars->k_empty[s], ph ^ 1);
                     ptx::mbar_expect_tx(&bars->k_full[s], KV_BYTES);
@@ -181,205 +149,118 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer (warp-uniform loops, one elected lane issues) ----------------
-        constexpr uint32_t idesc_pv = ptx::make_idesc_bf16(AT_M, HD) | ptx::kIdescBMajorMN;
-        const uint32_t tm_o = tmem_base + AT_O_COL;
-        // S_j = Q K_j^T into S buffer (jt & 1); jt counts this CTA's tiles across items; qb = the item's Q buffer
-        auto issue_qk = [&](int jt, int valid, bool last, int qb) {
-            const int s = jt % STAGES;
-            const uint32_t ph = (uint32_t)(jt / STAGES) & 1u;
-            const int n_j = valid >= AT_N ? AT_N : ((valid + 15) & ~15);         // keys of this tile, multiple of 16
-            const uint32_t q_addr = ptx::smem_u32(smem_q + qb * Q_BYTES);
-            const uint32_t k_addr = ptx::smem_u32(smem_k + s * KV_BYTES);
-            ptx::mbar_wait(&bars->k_full[s], ph);
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-                const uint32_t idesc_qk = ptx::make_idesc_bf16(AT_M, n_j);
-                const uint32_t tm_s = tmem_base + (uint32_t)((jt & 1) * AT_N);
-#pragma unroll
-                for (int kk = 0; kk < HD / 16; ++kk) {
-                    const uint32_t qoff = (uint32_t)((kk >> 2) * AT_BOX_BYTES + (kk & 3) * 32);
-                    const uint32_t koff = (uint32_t)((kk >> 2) * AT_KV_BOX_BYTES + (kk & 3) * 32);
-                    ptx::umma_f16_ss(tm_s, ptx::make_desc_sw128(q_addr + qoff), ptx::make_desc_sw128(k_addr + koff),
-                                     idesc_qk, (uint32_t)(kk != 0));
-                }
-                ptx::umma_commit(&bars->k_empty[s]);
-                if (last) ptx::umma_commit(&bars->q_empty[qb]);                  // the Q tile may be overwritten
-                ptx::umma_commit(&bars->s_full[jt & 1]);
-            }
-            __syncwarp();
-        };
-        int jt = 0, it = 0;
-        bool pre = false;                                 // this item's first QK^T was issued during the previous item
-        int4 cur = plan_at(blockIdx.x);
-        for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++it) {
-            const int4 nxt = plan_at(w + gridDim.x);
-            const bool has_next = w + gridDim.x < n_work;
-            const int len = cur.y;
-            cur = nxt;
-            const int n_kt = (len + AT_N - 1) / AT_N;
-            const int qb = it % QBUF;
-            if (!pre) {
-                ptx::mbar_wait(&bars->q_full[qb], (uint32_t)(it / QBUF) & 1u);
-                issue_qk(jt, len, n_kt == 1, qb);
-            }
-            pre = false;
-            for (int j = 0; j < n_kt; ++j, ++jt) {
-                // the next tile's scores first: they do not depend on this tile's softmax (other S buffer).  After the
-                // item's last tile that is the FIRST tile of the next item (its Q sits in the other Q buffer).
-                if (j + 1 < n_kt) {
-                    issue_qk(jt + 1, len - (j + 1) * AT_N, j + 2 == n_kt, qb);
-                } else if (QBUF == 2 && has_next) {
-                    const int len2 = nxt.y;
-                    const int qb2 = (it + 1) % QBUF;
-                    ptx::mbar_wait(&bars->q_full[qb2], (uint32_t)((it + 1) / QBUF) & 1u);
-                    issue_qk(jt + 1, len2, len2 <= AT_N, qb2);
-                    pre = true;
-                }
-                const int s = jt % STAGES;
-                const uint32_t ph = (uint32_t)(jt / STAGES) & 1u;
-                const int valid = len - j * AT_N;
-                const int n_j = valid >= AT_N ? AT_N : ((valid + 15) & ~15);
-                const uint32_t v_addr = ptx::smem_u32(smem_v + s * KV_BYTES);
-                ptx::mbar_wait(&bars->p_full[jt & 1], (uint32_t)(jt >> 1) & 1u);   // probabilities are in tensor memory
-                ptx::mbar_wait(&bars->v_full[s], ph);
-                ptx::tc_fence_after();
-                if (ptx::elect_one()) {
-                    const uint32_t tm_p = tmem_base + (uint32_t)((jt & 1) * AT_N);
-                    for (int i = 0; i < n_j / 16; ++i)
-                        ptx::umma_f16_ts(tm_o, tm_p + (uint32_t)(8 * i),
-                                         ptx::make_desc_sw128_mn(v_addr + (uint32_t)i * 2048u, AT_KV_BOX_BYTES), idesc_pv,
-                                         (uint32_t)((j | i) != 0));
-                    ptx::umma_commit(&bars->v_empty[s]);
-                    if (j == n_kt - 1) ptx::umma_commit(&bars->o_full);
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        // ---------------- softmax + epilogue: 4 warps, one per TMEM lane quadrant ----------------
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16);
-        const uint32_t o_col = (uint32_t)AT_O_COL;
-        int jt = 0, it = 0;
-        int4 cur = plan_at(blockIdx.x);
-        for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++it) {
-            const int4 nxt = plan_at(w + gridDim.x);
-            const int h = w / n_pairs;
-            const int lo = cur.x, len = cur.y, q0 = cur.z;
-            cur = nxt;
-            const int n_kt = (len + AT_N - 1) / AT_N;
-            float m_run = -INFINITY, l_run = 0.f;
-            for (int j = 0; j < n_kt; ++j, ++jt) {
-                const int valid = len - j * AT_N;
-                const uint32_t s_addr = lane_addr + (uint32_t)((jt & 1) * AT_N);
-                ptx::mbar_wait(&bars->s_full[jt & 1], (uint32_t)(jt >> 1) & 1u);   // also: every earlier O += P V retired
-                ptx::tc_fence_after();
-                // the row's 64 scores, read once (columns past the tile's keys hold stale data: masked, never used)
-                uint32_t r0[32], r1[32];
-                ptx::tmem_ld_32x32(s_addr, r0);
-                ptx::tmem_ld_32x32(s_addr + 32, r1);
-                ptx::tmem_ld_wait();
-                if (valid < AT_N) {                                // last tile of the sequence: mask the keys past it
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        r0[i] = i < valid ? r0[i] : 0xff800000u;   // -inf: exp2 gives 0
-                        r1[i] = 32 + i < valid ? r1[i] : 0xff800000u;
-                    }
-                }
-                // row maximum: four independent chains (one chain of 32 dependent FMNMX is ~130 cycles of pure latency
-                // in front of the exponentials)
-                float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                    mx4[i & 3] = fmaxf(mx4[i & 3], fmaxf(__uint_as_float(r0[i]), __uint_as_float(r1[i])));
-                const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-                float m_new = fmaxf(m_run, mx);
-                const bool grow = (m_new - m_run) * scale_log2 > AT_RESCALE_LOG2;   // true on the first tile (m_run = -inf)
-                if (!grow) m_new = m_run;
-                const float alpha = ex2_approx((m_run - m_new) * scale_log2);       // 1 when the maximum is kept
-                const bool rescale = j > 0 && __any_sync(0xffffffffu, grow);
-                l_run *= alpha;
-                m_run = m_new;
-                const float mb = m_new * scale_log2;
-                // probabilities, packed in place: pair (2i, 2i+1) -> 32-bit column i (reads run ahead of the writes)
-                float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float p0 = ex2_approx(fmaf(__uint_as_float(r0[2 * i]), scale_log2, -mb));
-                    const float p1 = ex2_approx(fmaf(__uint_as_float(r0[2 * i + 1]), scale_log2, -mb));
-                    l0 += p0; l1 += p1;
-                    __nv_bfloat162 v = __floats2bfloat162_rn(p0, p1);
-                    r0[i] = *reinterpret_cast<uint32_t*>(&v);
-                }
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float p0 = ex2_approx(fmaf(__uint_as_float(r1[2 * i]), scale_log2, -mb));
-                    const float p1 = ex2_approx(fmaf(__uint_as_float(r1[2 * i + 1]), scale_log2, -mb));
-                    l0 += p0; l1 += p1;
-                    __nv_bfloat162 v = __floats2bfloat162_rn(p0, p1);
-                    r0[16 + i] = *reinterpret_cast<uint32_t*>(&v);
-                }
-                l_run += l0 + l1;
-                ptx::tmem_st_32x32(s_addr, r0);                    // P over the first 32 columns of this S buffer
-                if (rescale) {
-                    // rare: bring the O columns to the new maximum (after the S registers are dead)
-#pragma unroll
-                    for (int c = 0; c < HD / 32; ++c) {
-                        uint32_t r[32];
-                        ptx::tmem_ld_32x32(lane_addr + o_col + c * 32, r);
-                        ptx::tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-                        ptx::tmem_st_32x32(lane_addr + o_col + c * 32, r);
-                    }
-                }
-                ptx::tmem_st_wait();
-                ptx::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&bars->p_full[jt & 1]);
-            }
-            // epilogue of the item: O / row sum -> bf16 -> global
-            const float inv = 1.0f / l_run;
-            ptx::mbar_wait(&bars->o_full, (uint32_t)it & 1u);
-            ptx::tc_fence_after();
-            const bool row_ok = q0 + row < len;
-            __nv_bfloat16* orow = out + (int64_t)(lo + q0 + row) * ldo + h * HD;
-#pragma unroll
-            for (int c = 0; c < HD / 32; ++c) {
-                uint32_t r[32];
-                ptx::tmem_ld_32x32(lane_addr + o_col + c * 32, r);
-                ptx::tmem_ld_wait();
-                if (row_ok) {
-#pragma unroll
-                    for (int i = 0; i < 32; i += 8) {
-                        uint4 pk;
-                        __nv_bfloat162 v;
-                        v = __floats2bfloat162_rn(__uint_as_float(r[i]) * inv, __uint_as_float(r[i + 1]) * inv);
-                        pk.x = *reinterpret_cast<uint32_t*>(&v);
-                        v = __floats2bfloat162_rn(__uint_as_float(r[i + 2]) * inv, __uint_as_float(r[i + 3]) * inv);
-                        pk.y = *reinterpret_cast<uint32_t*>(&v);
-                        v = __floats2bfloat162_rn(__uint_as_float(r[i + 4]) * inv, __uint_as_float(r[i + 5]) * inv);
-                        pk.z = *reinterpret_cast<uint32_t*>(&v);
-                        v = __floats2bfloat162_rn(__uint_as_float(r[i + 6]) * inv, __uint_as_float(r[i + 7]) * inv);
-                        pk.w = *reinterpret_cast<uint32_t*>(&v);
-                        *reinterpret_cast<uint4*>(orow + c * 32 + i) = pk;
-                    }
-                }
-            }
-            // the O columns are rewritten by the next item's first O = P V, which is issued only after this warp's
-            // next p_full arrival
-            ptx::tc_fence_before();
-        }
+        return;
     }
 
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<AT_TMEM_COLS>(tmem_base);
+    // ---------------- consumers: warpgroup cw owns query rows [64 cw, 64 cw + 64) of the item
+    const int cw = (threadIdx.x >> 7) - 1;
+    const int wq = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int r_in = cw * 64 + wq * 16 + (lane >> 2);    // this thread's rows r_in and r_in + 8 of the item
+    const uint32_t q_addr = ptx::smem_u32(smem_q) + (uint32_t)(cw * 64 * 128);
+    int jt = 0, it = 0;
+    int4 cur = plan_at(blockIdx.x);
+    for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++it) {
+        const int4 nxt = plan_at(w + gridDim.x);
+        const int h = w / n_pairs;
+        const int lo = cur.x, len = cur.y, q0 = cur.z;
+        cur = nxt;
+        const int n_kt = (len + AT_N - 1) / AT_N;
+        float o[HD / 2];
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+        float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        ptx::mbar_wait(&bars->q_full, (uint32_t)it & 1u);
+        for (int j = 0; j < n_kt; ++j, ++jt) {
+            const int s = jt % AT_STAGES;
+            const uint32_t ph = (uint32_t)(jt / AT_STAGES) & 1u;
+            const int valid = len - j * AT_N;
+            // ---- S = Q K^T (64 x 64 per warpgroup)
+            float sc[32];
+            const uint32_t k_addr = ptx::smem_u32(smem_k + s * KV_BYTES);
+            ptx::mbar_wait(&bars->k_full[s], ph);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < HD / 16; ++kk) {
+                const uint32_t qoff = (uint32_t)((kk >> 2) * AT_BOX_BYTES + (kk & 3) * 32);
+                const uint32_t koff = (uint32_t)((kk >> 2) * AT_KV_BOX_BYTES + (kk & 3) * 32);
+                ptx::wgmma_ss_n64(sc, ptx::make_desc_sw128(q_addr + qoff), ptx::make_desc_sw128(k_addr + koff),
+                                  (uint32_t)(kk != 0));
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+            ptx::fence_regs(sc);
+            if (leader) {
+                ptx::mbar_arrive(&bars->k_empty[s]);
+                if (j == n_kt - 1) ptx::mbar_arrive(&bars->q_empty);       // the Q tile may be overwritten
+            }
+            // ---- online softmax: keys past the sequence -> -inf; a row is spread over the 4 threads of a quad
+            const int c0 = (lane & 3) * 2;
+            if (valid < AT_N) {
+#pragma unroll
+                for (int i = 0; i < 32; ++i) {
+                    const int col = (i >> 2) * 8 + c0 + (i & 1);
+                    if (col >= valid) sc[i] = -INFINITY;
+                }
+            }
+            uint32_t pa[16];                             // P as bf16 A fragments: 4 k16 slices x 4 registers
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sc[4 * jj + 2 * hh], sc[4 * jj + 2 * hh + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                const float m_new = fmaxf(m_run[hh], mx);         // finite: every tile has >= 1 valid key
+                const float alpha = ex2_approx((m_run[hh] - m_new) * scale_log2);     // 0 on the first tile
+                m_run[hh] = m_new;
+                const float mb = m_new * scale_log2;
+                float l = 0.f;
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {
+                    const float p0 = ex2_approx(fmaf(sc[4 * jj + 2 * hh], scale_log2, -mb));
+                    const float p1 = ex2_approx(fmaf(sc[4 * jj + 2 * hh + 1], scale_log2, -mb));
+                    l += p0 + p1;
+                    // key columns 8 jj + c0 (+1): slice jj / 2, register (jj % 2) * 2 + hh
+                    pa[(jj >> 1) * 4 + (jj & 1) * 2 + hh] = pack_bf16x2(p0, p1);
+                }
+                l_run[hh] = l_run[hh] * alpha + l;
+#pragma unroll
+                for (int i = 0; i < HD / 8; ++i) {
+                    o[4 * i + 2 * hh] *= alpha;
+                    o[4 * i + 2 * hh + 1] *= alpha;
+                }
+            }
+            // ---- O += P V
+            const uint32_t v_addr = ptx::smem_u32(smem_v + s * KV_BYTES);
+            ptx::mbar_wait(&bars->v_full[s], ph);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < AT_N / 16; ++kk) {
+                const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+                const uint64_t db = ptx::make_desc_sw128_mn(v_addr + (uint32_t)kk * 2048u, AT_KV_BOX_BYTES);
+                if constexpr (HD == 64) ptx::wgmma_rs_n64_bmn(*reinterpret_cast<float(*)[32]>(o), a, db, 1u);
+                else ptx::wgmma_rs_n128_bmn(*reinterpret_cast<float(*)[64]>(o), a, db, 1u);
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+            ptx::fence_regs(o);
+            if (leader) ptx::mbar_arrive(&bars->v_empty[s]);
+        }
+        // ---- epilogue of the item: O / row sum -> bf16 -> global
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            float l = l_run[hh];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = 1.0f / l;
+            const int row = q0 + r_in + 8 * hh;
+            if (row >= len) continue;
+            __nv_bfloat16* orow = out + (int64_t)(lo + row) * ldo + h * HD + (lane & 3) * 2;
+#pragma unroll
+            for (int i = 0; i < HD / 8; ++i)
+                *reinterpret_cast<uint32_t*>(orow + 8 * i) = pack_bf16x2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+        }
     }
 }
 
@@ -387,7 +268,7 @@ int attn_bidir_legacy(const void* qkv, int64_t ld, const int32_t* cu_seqlens, in
                       int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, float softmax_scale, void* out, int64_t ldo,
                       cudaStream_t st);
 
-static int g_attn_kernel = 0;     // ezr_attn_set_kernel: 0 = tcgen05 (default), 1 = legacy mma.sync kernel (cross-checks)
+static int g_attn_kernel = 0;     // ezr_attn_set_kernel: 0 = wgmma (default), 1 = legacy mma.sync kernel (cross-checks)
 static thread_local const char* g_attn_last = "none";
 
 // plan buffer (query-block list) of the calling thread's device, grown on demand
@@ -398,13 +279,10 @@ static thread_local int g_plan_dev = -1;
 template <int HD>
 static int attn_tc_launch(const CUtensorMap& map_q, const CUtensorMap& map_kv, const int32_t* cu, int n_seq, int max_len,
                           int n_heads, int n_kv_heads, float scale_log2, __nv_bfloat16* out, int64_t ldo, cudaStream_t st) {
-    const size_t smem = 1024 + (size_t)(HD / 64) * (at_qbuf(HD) * AT_BOX_BYTES + 2 * at_stages(HD) * AT_KV_BOX_BYTES) +
-                        sizeof(AttnBarriers) + 64;
+    const size_t smem = 1024 + (size_t)(HD / 64) * (AT_BOX_BYTES + 2 * AT_STAGES * AT_KV_BOX_BYTES) + sizeof(AttnBarriers);
     static bool attr_done = false;
     if (!attr_done) {
-        EZR_CUDA(cudaFuncSetAttribute(attn_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        EZR_CUDA(cudaFuncSetAttribute(attn_tc_kernel<HD>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                      cudaSharedmemCarveoutMaxShared));
+        EZR_CUDA(cudaFuncSetAttribute(attn_wgmma_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done = true;
     }
     const int max_qb = (max_len + AT_M - 1) / AT_M;
@@ -425,8 +303,8 @@ static int attn_tc_launch(const CUtensorMap& map_q, const CUtensorMap& map_kv, c
     attn_plan_kernel<<<1, 256, 0, st>>>(cu, n_seq, plan, plan_n);
     EZR_LAUNCH_CHECK();
     const long long upper = (long long)n_seq * max_qb * n_heads;      // work items at most
-    const int grid = (int)(upper < 2ll * sm_count() ? upper : 2ll * sm_count());
-    attn_tc_kernel<HD><<<grid, AT_THREADS, smem, st>>>(map_q, map_kv, plan, plan_n, n_heads, n_kv_heads, scale_log2, out, ldo);
+    const int grid = (int)(upper < sm_count() ? upper : sm_count());
+    attn_wgmma_kernel<HD><<<grid, AT_THREADS, smem, st>>>(map_q, map_kv, plan, plan_n, n_heads, n_kv_heads, scale_log2, out, ldo);
     EZR_LAUNCH_CHECK();
     return EZR_OK;
 }
@@ -434,7 +312,7 @@ static int attn_tc_launch(const CUtensorMap& map_q, const CUtensorMap& map_kv, c
 }  // namespace ezr
 
 extern "C" int ezr_attn_set_kernel(int32_t which) {
-    EZR_CHECK_ARG(which == 0 || which == 1, "attn_set_kernel: 0 = tcgen05, 1 = legacy mma.sync");
+    EZR_CHECK_ARG(which == 0 || which == 1, "attn_set_kernel: 0 = wgmma, 1 = legacy mma.sync");
     ezr::g_attn_kernel = which;
     return EZR_OK;
 }
@@ -460,7 +338,7 @@ extern "C" int ezr_attn_bidir(const void* qkv, int64_t n_tokens, int64_t ld, con
         return attn_bidir_legacy(qkv, ld, cu_seqlens, n_seq, max_len, n_heads, n_kv_heads, head_dim, softmax_scale, out,
                                  ldo, st);
     }
-    g_attn_last = "tcgen05";
+    g_attn_last = "wgmma";
     CUtensorMap map_q, map_kv;
     const uint64_t width = (uint64_t)(n_heads + 2 * n_kv_heads) * head_dim;
     int rc = encode_tmap_2d_bf16(&map_q, qkv, width, (uint64_t)n_tokens, (uint64_t)ld, 64, AT_M);

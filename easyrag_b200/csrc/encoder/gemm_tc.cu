@@ -1,4 +1,4 @@
-// bf16 GEMM on tcgen05 / TMEM with fused epilogues, for the chunk-embedding forward pass.
+// bf16 GEMM on wgmma (Hopper warpgroup MMA) with fused epilogues, for the chunk-embedding forward pass.
 //
 //   out[M, N'] = epilogue( A[M, K] . W[N, K]^T + bias[N] ) (+ residual[M, N'])
 //
@@ -7,82 +7,49 @@
 // cuBLAS calls behind the reference's projections: Qwen2 q/k/v/o and SwiGLU MLP (modeling_qwen.py:261-263,
 // 319,186) and the BERT-shaped encoder's dense layers behind SentenceTransformer.encode (hf_embeddings.py:118-123).
 //
-// CTA PAIRS (cta_group::2).  A single-CTA tcgen05.mma 128 x 256 x 16 reads A (4 KB) and B (8 KB) from shared memory every
-// 128 cycles while TMA refills the same 12 KB: 192 B/clk against the 128 B/clk a shared memory delivers, i.e. a ceiling
-// of two thirds of the tensor peak (measured in round 2: tensor pipe 65% active at best, 1130 TFLOP/s on the
-// friendliest shape).  In pair mode one instruction spans the two CTAs of a cluster pair (M = 256, N = 256): each CTA
-// keeps its own 128 rows of A and only its HALF of the W tile (128 of the 256 rows) in shared memory -- 8 KB per 128
-// cycles -- and each CTA's tensor memory receives its 128 rows of the result.  The leader CTA (cluster rank 0) issues
-// the MMAs; both CTAs run their own TMA producer (own A tile + own W half, bytes counted on the leader's barrier) and
-// their own epilogue (remote arrive on the leader's accumulator-free barrier).
+// One CTA computes one 128 x 256 output tile.  Warpgroup 0 is the TMA producer (one thread; a 4-stage ring of 128 x 64
+// A tiles and 256 x 64 W tiles, 48 KB a stage); warpgroups 1 and 2 each own 64 rows of the tile and issue
+// wgmma.m64n256k16 from the ring into 128 fp32 accumulator registers per thread, keeping one k-chunk of MMAs in flight
+// while the previous stage is handed back to the producer.  The epilogue runs on the accumulator registers: bias /
+// GELU / SwiGLU / residual in fp32, bf16 pairs stored straight to global memory.  SwiGLU needs no exchange: the gate
+// column c and its "up" column c + 128 of a 256-column tile sit in the same thread.
 //
 // Tile order: N tiles fastest.  The activations of a 147k-token batch (226 MB at K = 768, 905 MB at K = 3072) do not fit
-// the L2, the weights (a few MB) do: with M fastest every N tile re-streamed all of A from HBM (9x for the QKV
-// projection); with N fastest the CTAs in flight cover ~16 M tiles x all N tiles, so an A tile is fetched from HBM once.
-//
-// Persistent, warp-specialised: warp 0 = TMA producer (ring of 128x64 A tiles and 128x64 W half-tiles, 6 or 5 stages),
-// warp 1 = tcgen05.mma issuer (leader CTA only; 256x256x16 per instruction over the pair, fp32 accumulation into one of
-// two 256-column TMEM stages), warps 2.. = epilogue (8 warps for the plain form, 16 for GELU / SwiGLU): tcgen05.ld with
-// one output row per thread, bias / GELU / SwiGLU / residual in fp32, bf16 blocks through a swizzled shared-memory
-// staging buffer and TMA stores, overlapping the next tile's MMAs.  Shared memory is used to the last KB
-// (ring + staging + bias slices + barriers = 231.6 KB of the 227 KB opt-in limit's 232,448 bytes).
+// the 50 MB L2, the weights (a few MB) do: with N fastest the CTAs in flight cover a few M tiles x all N tiles, so an A
+// tile is fetched from HBM about once.
 #include "../ezr_common.cuh"
 #include "../ptx.cuh"
-
-#ifndef EZR_GEMM_PROBE
-#define EZR_GEMM_PROBE 0       // tuning probes (variant builds only): 1 = epilogue without stores, 2 = no epilogue
-#endif
 
 namespace ezr {
 
 constexpr int GM = 128, GN = 256, GK = 64;
-constexpr int G_STAGES_MAX = 6;     // TMA ring: 6 stages of 32 KB beside 8 epilogue warps, 5 beside 16 (their staging buffers)
-constexpr int G_ACC = 2;
-// Epilogue warps: EW / 4 warps share a TMEM lane quadrant and split the tile's columns.  Measured per shape (M = 147k
-// rows, session 11): the plain epilogue is fastest with 8 warps + 6 ring stages (qkv 1380 vs 1324 TFLOP/s), the
-// GELU and SwiGLU epilogues -- whose math is what the tile waits for -- with 16 warps + 5 stages (1153 vs 1088, 1367 vs 996).
-__host__ __device__ constexpr int epi_warps(int epi) { return epi == 0 ? 8 : 16; }
-#ifndef EZR_GEMM_PLAIN_STAGES
-#define EZR_GEMM_PLAIN_STAGES 6      // tuning switch (variant builds)
-#endif
-__host__ __device__ constexpr int ring_stages(int epi) { return epi == 0 ? EZR_GEMM_PLAIN_STAGES : 5; }
-// epilogue staging (all warps): what the ring leaves of the 227 KB -- 32 KB beside 6 stages, 64 KB beside 5
-__host__ __device__ constexpr int staging_bytes(int stages) { return stages >= 6 ? 32768 : 65536; }
-constexpr int G_BIAS_BYTES = 2048;                       // bf16 bias slices of the epilogue warps
-constexpr int G_A_BYTES = GM * GK * 2;   // 16 KB
-constexpr int G_B_BYTES = (GN / 2) * GK * 2;   // 16 KB: this CTA's half of the 256-row W tile
-constexpr int G_CLUSTER = 2;             // CTAs of a pair
+constexpr int G_STAGES = 4;
+constexpr int G_THREADS = 384;                 // producer warpgroup + two consumer warpgroups
+constexpr int G_A_BYTES = GM * GK * 2;         // 16 KB
+constexpr int G_B_BYTES = GN * GK * 2;         // 32 KB
 
 enum { EPI_NONE = 0, EPI_GELU = 1, EPI_SWIGLU = 2 };
 
 struct GemmParams {
     int M, N, K;
-    int kps;                         // k-chunks (64-wide TMA boxes) per pipeline stage: 1 or 2
-    int n_stages;                    // ring stages / kps
     int tiles_m, tiles_n;
     const __nv_bfloat16* bias;       // [N] or null
     const __nv_bfloat16* residual;   // [M, ldr] or null
     int64_t ldr;
     __nv_bfloat16* out;              // [M, ldo]
     int64_t ldo;
-    int tma_out;                     // 1: the output goes through shared memory and TMA stores (ldo % 8 == 0, 16-byte aligned)
-    int smem_slack;                  // bytes the launch could spare for aligning the dynamic shared memory to 1024
 };
 
 struct GemmBarriers {
-    uint64_t full[G_STAGES_MAX];
-    uint64_t empty[G_STAGES_MAX];
-    uint64_t acc_full[G_ACC];
-    uint64_t acc_empty[G_ACC];
-    uint32_t tmem_base;
+    uint64_t full[G_STAGES];
+    uint64_t empty[G_STAGES];
 };
 
 // erf GELU (HF "gelu"): gelu(x) = 0.5 x (1 + erf(x / sqrt 2)).  erfc(|z|) = t (a1 + t (a2 + t (a3 + t (a4 + t a5)))) exp(-z^2),
 // t = 1 / (1 + p |z|) (Abramowitz & Stegun 7.1.26, |error| <= 1.5e-7), evaluated through erfc on BOTH sides so the
 // negative tail keeps its relative accuracy: x <= 0: 0.5 x erfc(|z|);  x > 0: x - 0.5 x erfc(z).  Against the float64
 // definition the fp32 evaluation is within 4.7e-7 absolute over [-12, 12] and 2.3e-4 relative wherever |gelu| > 1e-3 (the bf16 output rounds to 3.9e-3 relative).
-// 15 instructions with two MUFU ops (rcp, ex2); libdevice erff is ~26 FMA-pipe instructions per element, which made the
-// 128 x 256 GELU epilogue (8 warps) slower than the tile's MMAs: the FFN-up GEMM was epilogue-bound.
+// 15 instructions with two MUFU ops (rcp, ex2); libdevice erff is ~26 FMA-pipe instructions per element.
 __device__ __forceinline__ float gelu_erf(float x) {
     const float z = fabsf(x) * 0.70710678118654752f;
     float t, e;
@@ -102,345 +69,123 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// out[row, col], col and col + 1 (when inside the output): bf16 pair stores where the address allows, else scalar
+__device__ __forceinline__ void store_pair(__nv_bfloat16* o, bool pair_ok, bool second, float x0, float x1) {
+    if (pair_ok && second) {
+        *reinterpret_cast<__nv_bfloat162*>(o) = __floats2bfloat162_rn(x0, x1);
+    } else {
+        o[0] = __float2bfloat16(x0);
+        if (second) o[1] = __float2bfloat16(x1);
+    }
+}
+
 template <int EPI>
-__global__ void __launch_bounds__(64 + 32 * epi_warps(EPI), 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
-               const __grid_constant__ CUtensorMap map_o, const GemmParams p) {          // map_w: boxes of GN / 2 rows (this CTA's half of the W tile)
+__global__ void __launch_bounds__(G_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const GemmParams p) {
     extern __shared__ __align__(1024) unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     unsigned char* smem_a = smem;
-    constexpr int EW = epi_warps(EPI);
-    constexpr int G_STAGES = ring_stages(EPI);
     unsigned char* smem_b = smem + (size_t)G_STAGES * G_A_BYTES;
-    constexpr int G_ST_TOTAL = staging_bytes(G_STAGES);
-    unsigned char* smem_st = smem_b + (size_t)G_STAGES * G_B_BYTES;          // 1024-aligned: the rings are multiples of 16 KB
-    __nv_bfloat16* s_bias = reinterpret_cast<__nv_bfloat16*>(smem_st + G_ST_TOTAL);
-    GemmBarriers* bars = reinterpret_cast<GemmBarriers*>(smem_st + G_ST_TOTAL + G_BIAS_BYTES);
-    // the layout fills the 227 KB: the alignment slack is whatever the launch could spare (p.smem_slack)
-    if (threadIdx.x == 0 && (size_t)(smem - smem_dyn) > (size_t)p.smem_slack) __trap();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // work = super-tiles of (two M tiles) x (one N tile), walked by cluster pairs; this CTA owns M tile 2 * sm + rank
-    const int rank = (int)ptx::cluster_ctarank();
-    const int pair = blockIdx.x / G_CLUSTER, n_pairs = gridDim.x / G_CLUSTER;
-    const int super_m = (p.tiles_m + 1) / 2;
-    const int n_tiles = super_m * p.tiles_n;
+    GemmBarriers* bars = reinterpret_cast<GemmBarriers*>(smem_b + (size_t)G_STAGES * G_B_BYTES);
+    const int tn = blockIdx.x % p.tiles_n, tm = blockIdx.x / p.tiles_n;     // N tiles fastest: see the header
     const int kchunks = p.K / GK;
+    const int wg = threadIdx.x >> 7;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&map_a);
         ptx::prefetch_tensormap(&map_w);
-        ptx::prefetch_tensormap(&map_o);
-        for (int i = 0; i < G_STAGES; ++i) { ptx::mbar_init(&bars->full[i], 1); ptx::mbar_init(&bars->empty[i], 1); }
-        // acc_empty is only waited on in the leader: the epilogue warps of both CTAs of the pair arrive there
-        for (int i = 0; i < G_ACC; ++i) { ptx::mbar_init(&bars->acc_full[i], 1); ptx::mbar_init(&bars->acc_empty[i], EW * G_CLUSTER); }
+        for (int i = 0; i < G_STAGES; ++i) { ptx::mbar_init(&bars->full[i], 1); ptx::mbar_init(&bars->empty[i], 2); }
         ptx::fence_barrier_init();
     }
-    if (warp == 1) ptx::tmem_alloc_pair<G_ACC * GN>(&bars->tmem_base);
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::cluster_sync();                 // the peer's barriers exist before anything arrives on them
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = bars->tmem_base;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = pair; t < n_tiles; t += n_pairs) {
-                const int tn = t % p.tiles_n, tm = (t / p.tiles_n) * 2 + rank;     // N tiles fastest: see the header
-                for (int kc = 0; kc < kchunks; kc += p.kps) {
-                    ptx::mbar_wait(&bars->empty[stage], phase ^ 1);          // the pair's MMAs have released the stage
-                    // the leader's barrier counts the bytes of BOTH CTAs (own A tile + own W half each)
-                    if (rank == 0)
-                        ptx::mbar_expect_tx(&bars->full[stage], (uint32_t)(p.kps * G_CLUSTER * (G_A_BYTES + G_B_BYTES)));
-                    for (int j = 0; j < p.kps; ++j) {
-                        ptx::tma_load_2d_pair(smem_a + (size_t)(stage * p.kps + j) * G_A_BYTES, &map_a, &bars->full[stage],
-                                              (kc + j) * GK, tm * GM);
-                        ptx::tma_load_2d_pair(smem_b + (size_t)(stage * p.kps + j) * G_B_BYTES, &map_w, &bars->full[stage],
-                                              (kc + j) * GK, tn * GN + rank * (GN / 2));
-                    }
-                    if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-                }
+    if (wg == 0) {
+        ptx::regs_dealloc<40>();
+        if (threadIdx.x == 0) {
+            for (int kc = 0; kc < kchunks; ++kc) {
+                const int s = kc % G_STAGES;
+                ptx::mbar_wait(&bars->empty[s], ((uint32_t)(kc / G_STAGES) & 1u) ^ 1u);
+                ptx::mbar_expect_tx(&bars->full[s], (uint32_t)(G_A_BYTES + G_B_BYTES));
+                ptx::tma_load_2d(smem_a + (size_t)s * G_A_BYTES, &map_a, &bars->full[s], kc * GK, tm * GM);
+                ptx::tma_load_2d(smem_b + (size_t)s * G_B_BYTES, &map_w, &bars->full[s], kc * GK, tn * GN);
             }
         }
-    } else if (warp == 1) {
-        // LEADER CTA only.  Whole warp walks the loop (uniform control flow); one elected lane issues the tcgen05
-        // instructions, each spanning the pair (M = 256)
-        constexpr uint32_t idesc = ptx::make_idesc_bf16(GM * G_CLUSTER, GN);
-        const uint64_t a_desc0 = ptx::make_desc_sw128(ptx::smem_u32(smem_a));
-        const uint64_t b_desc0 = ptx::make_desc_sw128(ptx::smem_u32(smem_b));
-        int stage = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        for (int t = pair; rank == 0 && t < n_tiles; t += n_pairs, ++it) {
-            const int as = it % G_ACC;
-            const uint32_t aph = (uint32_t)(it / G_ACC) & 1u;
-            ptx::mbar_wait(&bars->acc_empty[as], aph ^ 1);                       // both CTAs' epilogues have drained it
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(as * GN);
-            for (int kc = 0; kc < kchunks; kc += p.kps) {
-                ptx::mbar_wait(&bars->full[stage], phase);
-                ptx::tc_fence_after();
-                const uint64_t a_desc = a_desc0 + (uint64_t)(stage * p.kps * (G_A_BYTES >> 4));
-                const uint64_t b_desc = b_desc0 + (uint64_t)(stage * p.kps * (G_B_BYTES >> 4));
-                if (ptx::elect_one()) {
-                    for (int j = 0; j < p.kps; ++j) {
-#pragma unroll
-                        for (int k4 = 0; k4 < GK / 16; ++k4)
-                            ptx::umma_f16_ss_pair(d_tmem, a_desc + (uint64_t)(j * (G_A_BYTES >> 4) + k4 * 2),
-                                                  b_desc + (uint64_t)(j * (G_B_BYTES >> 4) + k4 * 2), idesc,
-                                                  (uint32_t)((kc | j | k4) != 0));
-                    }
-                    ptx::umma_commit_pair(&bars->empty[stage], (uint16_t)0x3);    // frees the stage in both CTAs
-                    if (kc + p.kps >= kchunks) ptx::umma_commit_pair(&bars->acc_full[as], (uint16_t)0x3);   // both epilogues
-                }
-                __syncwarp();
-                if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else {
-        // ---------------- epilogue: EW warps, EW / 4 per TMEM lane quadrant, each owning a slice of the tile's columns.
-        // A warp works in BLOCKS of 32 rows x BW columns (BW = 64, or 32 when the slice is that narrow): the
-        // accumulator chunks are read from tensor memory (one row per lane), bias / GELU / SwiGLU / residual applied
-        // in fp32, the block packed to bf16 into the warp's staging buffer -- laid out in the TMA swizzle of the block's
-        // row width, so every 16-byte shared-memory access is conflict-free -- and written by ONE TMA store of full
-        // 64/128-byte row segments.  (Stores straight from the registers, one output row per lane and 16 bytes per
-        // instruction, touch 32 half-filled sectors per instruction and were measured as the limit of every K = 768
-        // shape: profiles/R2j_*.)  The residual takes the same road backwards: a COALESCED load (LPR lanes per row)
-        // into registers one block ahead, through the staging buffer, read back row-per-lane -- the row-per-lane global
-        // load it replaces cost 32 L1 wavefronts per instruction.  With NB = 2 staging buffers the store of block k
-        // drains under block k + 1.
-        constexpr int n_out_chunks = (EPI == EPI_SWIGLU) ? GN / 64 : GN / 32;   // 32 output columns per chunk
-        constexpr int cpw = n_out_chunks / (EW / 4);                            // chunks per warp and tile
-        constexpr int BW = cpw >= 2 ? 64 : 32;
-        constexpr int SUB = BW / 32, NBLK = cpw / SUB;
-        constexpr int ROWB = BW * 2, BUFB = 32 * ROWB;
-        constexpr int ST_W = G_ST_TOTAL / EW, NB = ST_W / BUFB;
-        constexpr int LPR = BW / 8, RPI = 32 / LPR;                             // residual load: lanes per row, rows per instruction
-        constexpr bool kResStage = (EW == 8);            // the 16-warp forms (96 registers) keep the direct residual path
-        constexpr int kBiasPerWarp = cpw * 32 * (EPI == EPI_SWIGLU ? 2 : 1);
-        static_assert(NB >= 1 && NB <= 2 && cpw % SUB == 0 && kBiasPerWarp * EW * 2 <= G_BIAS_BYTES, "epilogue layout");
-        const int ew = warp - 2, quad = warp & 3, part = ew >> 2;
-        unsigned char* st0 = smem_st + (size_t)ew * ST_W;
-        __nv_bfloat16* sb = s_bias + ew * kBiasPerWarp;
-        const int n_out = (EPI == EPI_SWIGLU) ? p.N / 2 : p.N;
-        const int sw_own = BW == 64 ? (lane & 7) : ((lane >> 1) & 3);           // swizzle term of this lane's own row
-        const int ld_row = lane / LPR, ld_ch = lane % LPR;
-        const bool res_on = p.residual != nullptr;
-        const bool res_stage = kResStage && res_on && p.tma_out && (p.ldr % 8 == 0) && (n_out % 8 == 0) &&
-                               ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0);
-        int it = 0, seq = 0;                             // seq: blocks this warp has staged (buffer = seq % NB)
-        for (int t = pair; t < n_tiles; t += n_pairs, ++it) {
-            const int tn = t % p.tiles_n, tm = (t / p.tiles_n) * 2 + rank;     // N tiles fastest: see the header
-            const int as = it % G_ACC;
-            const uint32_t aph = (uint32_t)(it / G_ACC) & 1u;
-            const int row0 = tm * GM + quad * 32;
-            const int row = row0 + lane;
-            const bool row_ok = row < p.M;
-            const int c0 = part * cpw;
-            const int ocol_base = (EPI == EPI_SWIGLU) ? tn * (GN / 2) : tn * GN;
-            // bias: columns [c0 * 32, (c0 + cpw) * 32) of the tile (and the matching "up" columns for SwiGLU), as bf16
-            if (p.bias) {
-                __syncwarp();
-                for (int i = lane; i < cpw * 32; i += 32) {
-                    const int col = tn * GN + c0 * 32 + i;
-                    sb[i] = col < p.N ? p.bias[col] : __float2bfloat16(0.f);
-                    if (EPI == EPI_SWIGLU) {
-                        const int col2 = col + GN / 2;
-                        sb[cpw * 32 + i] = col2 < p.N ? p.bias[col2] : __float2bfloat16(0.f);
-                    }
-                }
-                __syncwarp();
-            }
-            uint4 rn[LPR];
-            auto load_res = [&](int tile_ocol_base, int tile_row0, int b) {
-                const int oc = tile_ocol_base + (c0 + b * SUB) * 32 + ld_ch * 8;
-#pragma unroll
-                for (int i = 0; i < LPR; ++i) {
-                    const int r = tile_row0 + ld_row + i * RPI;
-                    rn[i] = (r < p.M && oc + 8 <= n_out)
-                                ? __ldg(reinterpret_cast<const uint4*>(p.residual + (int64_t)r * p.ldr + oc))
-                                : make_uint4(0u, 0u, 0u, 0u);
-                }
-            };
-            if (kResStage && res_stage) load_res(ocol_base, row0, 0);
-            // the NEXT tile's residual block of this lane's row: pull it into L2 now, a whole tile ahead (the register
-            // loads run one block ahead, which covers an L2 hit but not a DRAM miss)
-            if (res_on && t + n_pairs < n_tiles) {
-                const int t2 = t + n_pairs;
-                const int row2 = ((t2 / p.tiles_n) * 2 + rank) * GM + quad * 32 + lane;
-                const int oc2 = ((EPI == EPI_SWIGLU) ? (t2 % p.tiles_n) * (GN / 2) : (t2 % p.tiles_n) * GN) + c0 * 32;
-                if (row2 < p.M && oc2 < n_out) {
-                    const char* a2 = reinterpret_cast<const char*>(p.residual + (int64_t)row2 * p.ldr + oc2);
-#pragma unroll
-                    for (int off = 0; off < cpw * 64; off += 128)
-                        asm volatile("prefetch.global.L2 [%0];" ::"l"(a2 + off));
-                }
-            }
-
-            ptx::mbar_wait(&bars->acc_full[as], aph);
-            ptx::tc_fence_after();
-#if EZR_GEMM_PROBE == 2
-            // tuning probe (never in the shipped build): no epilogue at all -> the TMA + MMA rate alone
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive_remote(&bars->acc_empty[as], 0u);
-            continue;
-#endif
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * GN);
-            // NOT unrolled: inlined copies of the block body are >130 KB of SASS (230 KB with GELU) and stream
-            // through the instruction cache on every tile.
-#pragma unroll 1
-            for (int b = 0; b < NBLK; ++b, ++seq) {
-                unsigned char* buf = st0 + (size_t)(seq % NB) * BUFB;
-                const int cb = c0 + b * SUB;
-                const int ocol = ocol_base + cb * 32;
-                const bool live = ocol < n_out;          // warp-uniform: the block has columns inside the output
-                bool buf_free = false;
-                if (kResStage && res_stage && live) {
-                    // the buffer is free once the store that last used it has READ it (not: reached memory)
-                    if (lane == 0) ptx::tma_store_wait_read<NB - 1>();
-                    __syncwarp();
-                    buf_free = true;
-#pragma unroll
-                    for (int i = 0; i < LPR; ++i) {
-                        const int r = ld_row + i * RPI;
-                        const int swz = BW == 64 ? (r & 7) : ((r >> 1) & 3);
-                        *reinterpret_cast<uint4*>(buf + r * ROWB + ((ld_ch ^ swz) << 4)) = rn[i];
-                    }
-                    __syncwarp();
-                }
-                uint32_t pk[SUB][16];
-#pragma unroll
-                for (int sidx = 0; sidx < SUB; ++sidx) {
-                    const int ci = b * SUB + sidx;       // chunk within this warp's slice
-                    const int c = c0 + ci;
-                    uint32_t r[32];
-                    float v[32];
-                    ptx::tmem_ld_32x32(taddr + c * 32, r);
-                    if (kResStage && sidx == 0 && res_stage && b + 1 < NBLK) load_res(ocol_base, row0, b + 1);
-                    if (EPI == EPI_SWIGLU) {
-                        uint32_t r2[32];
-                        ptx::tmem_ld_32x32(taddr + GN / 2 + c * 32, r2);
-                        ptx::tmem_ld_wait();
-#pragma unroll
-                        for (int j8 = 0; j8 < 4; ++j8) {
-                            uint4 bg = make_uint4(0u, 0u, 0u, 0u), bu = make_uint4(0u, 0u, 0u, 0u);
-                            if (p.bias) {
-                                bg = *reinterpret_cast<const uint4*>(sb + ci * 32 + j8 * 8);
-                                bu = *reinterpret_cast<const uint4*>(sb + cpw * 32 + ci * 32 + j8 * 8);
-                            }
-                            const __nv_bfloat16* hg = reinterpret_cast<const __nv_bfloat16*>(&bg);
-                            const __nv_bfloat16* hu = reinterpret_cast<const __nv_bfloat16*>(&bu);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float g = __uint_as_float(r[j8 * 8 + j]) + __bfloat162float(hg[j]);
-                                const float u = __uint_as_float(r2[j8 * 8 + j]) + __bfloat162float(hu[j]);
-                                v[j8 * 8 + j] = silu(g) * u;
-                            }
-                        }
-                    } else {
-                        ptx::tmem_ld_wait();
-#pragma unroll
-                        for (int j8 = 0; j8 < 4; ++j8) {
-                            uint4 b4 = make_uint4(0u, 0u, 0u, 0u);
-                            if (p.bias) b4 = *reinterpret_cast<const uint4*>(sb + ci * 32 + j8 * 8);
-                            const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&b4);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                float x = __uint_as_float(r[j8 * 8 + j]) + __bfloat162float(hb[j]);
-                                if (EPI == EPI_GELU) x = gelu_erf(x);
-                                v[j8 * 8 + j] = x;
-                            }
-                        }
-                    }
-                    if (b == NBLK - 1 && sidx == SUB - 1) {          // the tile's last read of tensor memory
-                        ptx::tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) ptx::mbar_arrive_remote(&bars->acc_empty[as], 0u);      // the leader's barrier
-                    }
-                    const int oc_s = ocol + sidx * 32;
-                    if (kResStage && res_stage) {
-                        if (live) {
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4) {
-                                const uint4 q4 = *reinterpret_cast<const uint4*>(buf + lane * ROWB + (((sidx * 4 + j4) ^ sw_own) << 4));
-                                const __nv_bfloat16* rh = reinterpret_cast<const __nv_bfloat16*>(&q4);
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) v[j4 * 8 + j] += __bfloat162float(rh[j]);
-                            }
-                        }
-                    } else if (res_on && row_ok && oc_s < n_out) {
-                        const __nv_bfloat16* rr = p.residual + (int64_t)row * p.ldr + oc_s;
-                        if (oc_s + 32 <= n_out && (p.ldr % 8 == 0) && ((reinterpret_cast<uintptr_t>(rr) & 15) == 0)) {
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4) {
-                                const uint4 q4 = __ldg(reinterpret_cast<const uint4*>(rr) + j4);
-                                const __nv_bfloat16* rh = reinterpret_cast<const __nv_bfloat16*>(&q4);
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) v[j4 * 8 + j] += __bfloat162float(rh[j]);
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                if (oc_s + j < n_out) v[j] += __bfloat162float(rr[j]);
-                        }
-                    }
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) pk[sidx][j] = pack_bf16(v[2 * j], v[2 * j + 1]);
-                }
-#if EZR_GEMM_PROBE == 1
-                if (p.M < 0) {                                  // tuning probe: the epilogue's math without its stores
-#else
-                if (p.tma_out) {
-#endif
-                    if (live) {
-                        if (!buf_free) {
-                            if (lane == 0) ptx::tma_store_wait_read<NB - 1>();
-                            __syncwarp();
-                        }
-#pragma unroll
-                        for (int sidx = 0; sidx < SUB; ++sidx)
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4)
-                                *reinterpret_cast<uint4*>(buf + lane * ROWB + (((sidx * 4 + j4) ^ sw_own) << 4)) =
-                                    make_uint4(pk[sidx][j4 * 4], pk[sidx][j4 * 4 + 1], pk[sidx][j4 * 4 + 2], pk[sidx][j4 * 4 + 3]);
-                        ptx::fence_proxy_async();                // generic-proxy writes -> visible to the TMA engine
-                        __syncwarp();
-                        if (lane == 0) {                         // rows past M and columns past n_out are clipped by the map
-                            ptx::tma_store_2d(&map_o, buf, ocol, row0);
-                            ptx::tma_store_commit();
-                        }
-                    }
-                } else if (row_ok && live) {
-#pragma unroll
-                    for (int sidx = 0; sidx < SUB; ++sidx) {
-                        const int oc_s = ocol + sidx * 32;
-                        __nv_bfloat16* op = p.out + (int64_t)row * p.ldo + oc_s;
-                        if (oc_s + 32 <= n_out && ((reinterpret_cast<uintptr_t>(op) & 15) == 0)) {
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4)
-                                *reinterpret_cast<uint4*>(op + j4 * 8) =
-                                    make_uint4(pk[sidx][j4 * 4], pk[sidx][j4 * 4 + 1], pk[sidx][j4 * 4 + 2], pk[sidx][j4 * 4 + 3]);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                if (oc_s + j < n_out)
-                                    op[j] = reinterpret_cast<const __nv_bfloat16*>(&pk[sidx][j >> 1])[j & 1];
-                        }
-                    }
-                }
-            }
-        }
-        if (lane == 0) ptx::tma_store_wait<0>();         // this warp's stores have left shared memory and are complete
+        return;
     }
+    ptx::regs_alloc<232>();
+    const int cw = wg - 1;                                   // this warpgroup's 64 rows of the tile
+    const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    const uint32_t a0 = ptx::smem_u32(smem_a) + (uint32_t)(cw * 64 * 128);
+    const uint32_t b0 = ptx::smem_u32(smem_b);
+    for (int kc = 0; kc < kchunks; ++kc) {
+        const int s = kc % G_STAGES;
+        ptx::mbar_wait(&bars->full[s], (uint32_t)(kc / G_STAGES) & 1u);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k4 = 0; k4 < GK / 16; ++k4)
+            ptx::wgmma_ss_n256(acc, ptx::make_desc_sw128(a0 + (uint32_t)(s * G_A_BYTES + k4 * 32)),
+                               ptx::make_desc_sw128(b0 + (uint32_t)(s * G_B_BYTES + k4 * 32)), (uint32_t)((kc | k4) != 0));
+        ptx::wgmma_commit();
+        if (kc > 0) {                                        // the previous chunk's MMAs are done: hand its stage back
+            ptx::wgmma_wait<1>();
+            if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&bars->empty[(kc - 1) % G_STAGES]);
+        }
+    }
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(acc);
+    // (the last stage is never handed back: no later load of this CTA needs it)
 
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::cluster_sync();                 // no CTA leaves (or frees tensor memory) while the pair's MMAs / arrivals are in flight
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc_pair<G_ACC * GN>(tmem_base);
+    // ---------------- epilogue on the accumulator registers
+    const int n_out = (EPI == EPI_SWIGLU) ? p.N / 2 : p.N;
+    const bool out_pair = (p.ldo % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 3) == 0);
+    const bool res_pair = p.residual && (p.ldr % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0);
+    const int cq = (lane & 3) * 2;
+    constexpr int NJ = (EPI == EPI_SWIGLU) ? GN / 16 : GN / 8;       // 8-column groups of output per thread row
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = tm * GM + cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        if (row >= p.M) continue;
+        __nv_bfloat16* orow = p.out + (int64_t)row * p.ldo;
+        const __nv_bfloat16* rrow = p.residual ? p.residual + (int64_t)row * p.ldr : nullptr;
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+            const int col = tn * GN + j * 8 + cq;                       // accumulator column (gate column for SwiGLU)
+            const int ocol = (EPI == EPI_SWIGLU) ? tn * (GN / 2) + j * 8 + cq : col;
+            if (ocol >= n_out) continue;
+            const bool second = ocol + 1 < n_out;
+            float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+            if (EPI == EPI_SWIGLU) {
+                float u0 = acc[4 * (j + NJ) + 2 * h], u1 = acc[4 * (j + NJ) + 2 * h + 1];
+                if (p.bias) {
+                    x0 += __bfloat162float(p.bias[col]);
+                    x1 += __bfloat162float(p.bias[col + 1]);
+                    u0 += __bfloat162float(p.bias[col + GN / 2]);
+                    u1 += __bfloat162float(p.bias[col + GN / 2 + 1]);
+                }
+                x0 = silu(x0) * u0;
+                x1 = silu(x1) * u1;
+            } else {
+                if (p.bias) {
+                    x0 += __bfloat162float(p.bias[col]);
+                    if (second) x1 += __bfloat162float(p.bias[col + 1]);
+                }
+                if (EPI == EPI_GELU) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
+            }
+            if (rrow) {
+                if (res_pair && second) {
+                    const float2 r2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(rrow + ocol));
+                    x0 += r2.x;
+                    x1 += r2.y;
+                } else {
+                    x0 += __bfloat162float(rrow[ocol]);
+                    if (second) x1 += __bfloat162float(rrow[ocol + 1]);
+                }
+            }
+            store_pair(orow + ocol, out_pair, second, x0, x1);
+        }
     }
 }
 
@@ -458,56 +203,24 @@ static int gemm_launch(const __nv_bfloat16* A, int M, int K, int64_t lda, const 
     p.tiles_m = (M + GM - 1) / GM;
     p.tiles_n = (N + GN - 1) / GN;
     p.bias = bias; p.residual = residual; p.ldr = ldr; p.out = out; p.ldo = ldo;
-    p.kps = 1;            // 2 chunks per stage was measured slower (coarser producer/consumer hand-off)
-    const int stages = epi == EPI_NONE ? ring_stages(EPI_NONE) : ring_stages(EPI_GELU);
-    const int ew = epi == EPI_NONE ? epi_warps(EPI_NONE) : epi_warps(EPI_GELU);
-    static_assert(ring_stages(EPI_GELU) == ring_stages(EPI_SWIGLU) && epi_warps(EPI_GELU) == epi_warps(EPI_SWIGLU), "");
-    p.n_stages = stages / p.kps;
-    const int n_out = epi == EPI_SWIGLU ? N / 2 : N;
-    p.tma_out = (ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) ? 1 : 0;
-    CUtensorMap map_a, map_w, map_o;
+    CUtensorMap map_a, map_w;
     int rc = encode_tmap_2d_bf16(&map_a, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, GK, GM);
     if (rc) return rc;
-    rc = encode_tmap_2d_bf16(&map_w, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, GK, GN / G_CLUSTER);
+    rc = encode_tmap_2d_bf16(&map_w, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, GK, GN);
     if (rc) return rc;
-    // output map: boxes of BW columns x 32 rows (one epilogue warp's block), swizzle = the block's row bytes.  Without
-    // TMA stores the kernel never touches it; it is then encoded over A so that the argument stays a valid descriptor.
-    const int cpw = (epi == EPI_SWIGLU ? GN / 64 : GN / 32) / (ew / 4);
-    const int bw = cpw >= 2 ? 64 : 32;                    // block width of the kernel's epilogue (see there)
-    if (p.tma_out) rc = encode_tmap_2d_bf16(&map_o, out, (uint64_t)n_out, (uint64_t)M, (uint64_t)ldo, (uint32_t)bw, 32, bw * 2);
-    else map_o = map_a;
-    if (rc) return rc;
-    const size_t need = (size_t)stages * (G_A_BYTES + G_B_BYTES) + (size_t)staging_bytes(stages) + G_BIAS_BYTES +
-                        sizeof(GemmBarriers);
-    const size_t kMaxSmem = 232448;                       // 227 KB opt-in limit of sm_100
-    EZR_CHECK_ARG(need <= kMaxSmem, "gemm: shared-memory layout of %zu bytes does not fit", need);
-    p.smem_slack = (int)(kMaxSmem - need < 1023 ? kMaxSmem - need : 1023);
-    const size_t smem = need + (size_t)p.smem_slack;
-    typedef void (*kern_t)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmParams);
-    static const kern_t table[3] = {gemm_tc_kernel<EPI_NONE>, gemm_tc_kernel<EPI_GELU>, gemm_tc_kernel<EPI_SWIGLU>};
+    const size_t smem = 1024 + (size_t)G_STAGES * (G_A_BYTES + G_B_BYTES) + sizeof(GemmBarriers);
+    typedef void (*kern_t)(const CUtensorMap, const CUtensorMap, const GemmParams);
+    static const kern_t table[3] = {gemm_wgmma_kernel<EPI_NONE>, gemm_wgmma_kernel<EPI_GELU>, gemm_wgmma_kernel<EPI_SWIGLU>};
     static bool attr_done[3] = {false, false, false};
     if (!attr_done[epi]) {
         EZR_CUDA(cudaFuncSetAttribute(table[epi], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done[epi] = true;
     }
-    const int n_super = ((p.tiles_m + 1) / 2) * p.tiles_n;           // (two M tiles) x (one N tile) per cluster pair
-    int pairs = sm_count() / G_CLUSTER;
-    if (n_super < pairs) pairs = n_super;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(pairs * G_CLUSTER));
-    cfg.blockDim = dim3((unsigned)(64 + 32 * ew));
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = G_CLUSTER;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    const long long tiles = (long long)p.tiles_m * p.tiles_n;
+    EZR_CHECK_ARG(tiles < (1ll << 31), "gemm: too many tiles");
     {
         ProfScope prof(EZR_PROF_ENC_GEMM, st);
-        EZR_CUDA(cudaLaunchKernelEx(&cfg, table[epi], map_a, map_w, map_o, p));
+        table[epi]<<<(unsigned)tiles, G_THREADS, smem, st>>>(map_a, map_w, p);
     }
     EZR_LAUNCH_CHECK();
     return EZR_OK;

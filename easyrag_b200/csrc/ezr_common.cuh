@@ -1,4 +1,4 @@
-// Common device/host helpers for the easyrag_b200 kernels (sm_100a only).
+// Common device/host helpers for the easyrag_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

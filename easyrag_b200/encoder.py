@@ -4,7 +4,7 @@ Replaces the model call inside ``GTEEmbedding._embed`` (gte_embeddings.py:59-72 
 ``Qwen2Model.forward`` run bidirectionally, modeling_qwen.py:956-1116) and inside
 ``HuggingFaceEmbedding._embed`` (hf_embeddings.py:112-123 -> SentenceTransformer.encode on a BERT
 encoder).  The host code is Python, as in the reference; every arithmetic step is a CUDA kernel behind
-the C ABI (csrc/encoder/*.cu): tcgen05 GEMMs with fused bias / GELU / SwiGLU / residual epilogues,
+the C ABI (csrc/encoder/*.cu): wgmma GEMMs with fused bias / GELU / SwiGLU / residual epilogues,
 tensor-core bidirectional attention over packed sequences, RMSNorm / LayerNorm / RoPE / pooling kernels.
 torch tensors are only the device buffers.
 

@@ -1,5 +1,5 @@
 /*
- * easyrag_b200 -- C ABI of the B200-native coarse-ranking path.
+ * easyrag_b200 -- C ABI of the H100-native coarse-ranking path.
  *
  * The reference (BUAADreamer/EasyRAG) has no native code and therefore no FFI
  * for this path: its boundary is the Python class surface of
@@ -19,7 +19,7 @@
  *     `id_base` is added on output so a row-sharded corpus yields global ids.
  *   - canonical rank order everywhere: score descending, then id descending
  *     (== numpy argsort(kind="stable")[::-1], SURVEY.md 8(c)).
- *   - the library targets sm_100a only; ezr_device_check() fails elsewhere.
+ *   - the library targets sm_90a only; ezr_device_check() fails elsewhere.
  */
 #ifndef EASYRAG_B200_H
 #define EASYRAG_B200_H
@@ -134,8 +134,8 @@ int ezr_bm25_term_max(const int64_t* indptr, const uint32_t* post_pk, int32_t vo
                       void* stream);
 
 /* 1: the candidate pass of ezr_bm25_topk may skip non-essential terms when the index carries term_max;
- * 0 (default): it reads every posting.  Results are identical either way; on the measured workload the extra
- * candidates cost more rescoring time than the skipped postings save (profiles/README.md), hence the default. */
+ * 0 (default): it reads every posting.  Results are identical either way; the extra candidates it produces
+ * cost rescoring time that can exceed what the skipped postings save, hence the default. */
 int ezr_bm25_set_skipping(int32_t on);
 
 /* 1 (default): every candidate launch is preceded by a plan kernel that resolves token -> posting segment for all its
@@ -205,22 +205,22 @@ int ezr_dense_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t
  * in elements; out may be a slice of a larger preallocated corpus matrix (append without rebuilding). */
 int ezr_normalize_rows(const void* x, int32_t x_is_f32, int64_t ldx, int64_t n_rows, int32_t dim, void* out_bf16,
                        int64_t ldo, void* stream);
-/* 0 = pick automatically, 1 = force the generic SIMT kernel, 2 = force tcgen05 with the query block in shared
- * memory (SS), 3 = force tcgen05 with the query block in tensor memory (TS) and 64-row corpus tiles, 4 = TS with
- * 128-row corpus tiles (the automatic choice), 5 = 4 run in cluster pairs (two neighbouring query blocks on the same
- * corpus split; each CTA loads half of every corpus tile and TMA-multicasts it to both); 2-5 error if the shape is
- * unsupported */
+/* 0 = pick automatically, 1 = force the generic SIMT kernel, 2 = force the wgmma kernel with 128-query blocks
+ * (dim <= 768; the automatic choice there), 3 = force the wgmma kernel with 64-query blocks (the automatic choice
+ * above 768), 4 = 64-query blocks and 128-row corpus tiles, 5 = 4 run in cluster pairs (two neighbouring query blocks
+ * on the same corpus split; each CTA loads half of every corpus tile and TMA-multicasts it to both); 2-5 error if the
+ * shape is unsupported */
 int ezr_dense_set_kernel(int32_t which);
 /* name of the kernel the last ezr_dense_topk call on this thread launched
- * ("tcgen05" / "tcgen05-ts" / "tcgen05-ts128" / "tcgen05-ts128-mc2" / "simt") */
+ * ("wgmma" / "wgmma-q64" / "wgmma-q64-n128" / "wgmma-q64-n128-mc2" / "simt") */
 const char* ezr_dense_last_kernel(void);
 
-/* Cap the TMA ring of the tcgen05 kernels at `stages` stages (0 = use all shared memory, the default).  A capped
- * ring leaves shared memory on every SM for kernels of another stream: CoarseRanker(overlap=True) uses it to let
- * BM25 CTAs co-reside with the persistent dense CTA (tensor pipe vs. integer/issue bound work). */
+/* Cap the TMA ring of the wgmma kernel at `stages` stages (0 = use all shared memory, the default).  A capped
+ * ring leaves shared memory on an SM for kernels of another stream only when the resident query block is small; a
+ * 128-query block of dim 768 fills the SM either way, and the cap then only shortens the ring. */
 int ezr_dense_set_stage_cap(int32_t stages);
 
-/* Measurement probes for the tcgen05 TS kernel (results become garbage; never use outside bench experiments):
+/* Measurement probes for the wgmma kernel (results become garbage; never use outside bench experiments):
  * bit mask: 1 = pipeline without TMA loads, 2 = one k-chunk of MMAs per tile, 4 = epilogue without the
  * insertion path. */
 int ezr_dense_set_probe(int32_t probe);
@@ -276,20 +276,20 @@ int ezr_rerank_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32
  * [cu_seqlens[b], cu_seqlens[b+1]) -- no padding tokens.  The Python classes in easyrag_b200/encoder.py chain
  * these per layer on one stream. */
 
-/* out[M,N'] = epi(A[M,K] . W[N,K]^T + bias) (+ residual); tcgen05/TMEM/TMA.  epilogue: 0 none, 1 GELU(erf),
+/* out[M,N'] = epi(A[M,K] . W[N,K]^T + bias) (+ residual); wgmma + TMA.  epilogue: 0 none, 1 GELU(erf),
  * 2 SwiGLU (W rows interleaved per 256: 128 gate rows then the matching 128 up rows; N' = N/2).  K % 64 == 0. */
 int ezr_gemm_bf16(const void* a, int32_t m, int32_t k, int64_t lda, const void* w, int32_t n, int64_t ldw,
                   const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo, int32_t epilogue,
                   void* stream);
 /* non-causal attention over packed q|k|v rows ([n_tokens, (H + 2*KV) * hd], row stride ld); head_dim 64 or 128; GQA
- * via n_kv_heads.  Default kernel: tcgen05 (S = QK^T and O += PV on the 5th-gen tensor cores, S/P/O in tensor memory,
+ * via n_kv_heads.  Default kernel: wgmma (S = QK^T and O += PV on the tensor cores, S/P/O in registers,
  * Q/K/V tiles by TMA).  n_tokens bounds the TMA tensor map (tiles that run past the last token are zero-filled). */
 int ezr_attn_bidir(const void* qkv, int64_t n_tokens, int64_t ld, const int32_t* cu_seqlens, int32_t n_seq,
                    int32_t max_len, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, float softmax_scale, void* out,
                    int64_t ldo, void* stream);
-/* 0 = tcgen05 kernel (default), 1 = the warp-level mma.sync kernel it replaced (kept as an independent cross-check) */
+/* 0 = wgmma kernel (default), 1 = the warp-level mma.sync kernel (kept as an independent cross-check) */
 int ezr_attn_set_kernel(int32_t which);
-/* "tcgen05" / "mma.sync": what the last ezr_attn_bidir call on this thread launched */
+/* "wgmma" / "mma.sync": what the last ezr_attn_bidir call on this thread launched */
 const char* ezr_attn_last_kernel(void);
 int ezr_embed_gather(const int32_t* ids, int32_t n_tokens, const void* table, int64_t ldt, int32_t vocab, int32_t dim,
                      void* out, int64_t ldo, void* stream);
@@ -319,7 +319,7 @@ int ezr_pool_normalize(const void* hidden, int64_t ldh, const int32_t* cu_seqlen
  * kernel launches recorded in `slot` since the last reset. */
 typedef enum ezr_prof_slot {
     EZR_PROF_BM25_SCORE = 0, /* bm25_score_kernel (fused top-k or score rows) */
-    EZR_PROF_DENSE_TC = 1,   /* dense_tc_kernel (tcgen05) */
+    EZR_PROF_DENSE_TC = 1,   /* dense_wgmma_kernel */
     EZR_PROF_DENSE_SIMT = 2, /* dense_scores_simt_kernel */
     EZR_PROF_MERGE = 3,      /* merge / select kernels */
     EZR_PROF_FUSE = 4,       /* rrf / simple fusion */

@@ -1,5 +1,5 @@
 """Overlay of the reference's ``easyrag`` package: put this directory's parent (``<repo>/shim``) on ``sys.path``
-BEFORE the reference's ``src`` and ``pipeline/pipeline.py`` runs unchanged against the B200 classes.
+BEFORE the reference's ``src`` and ``pipeline/pipeline.py`` runs unchanged against the H100 classes.
 
 ``pipeline.py:15,19`` import ``..custom.embeddings`` and ``..custom.retrievers`` relative to the ``easyrag``
 package.  This package extends its search path with every other ``easyrag`` directory on ``sys.path`` (the

@@ -1,4 +1,4 @@
-"""GPU: embedding forward pass (tcgen05 GEMMs, attention, norms, pooling) vs PyTorch fp32 and vs the reference model.
+"""GPU: embedding forward pass (wgmma GEMMs, attention, norms, pooling) vs PyTorch fp32 and vs the reference model.
 
 Tolerances: the north star allows 1e-3 on cosine scores for the bf16 embedding path; per-op checks compare the
 bf16 kernels with an fp32 evaluation of the same bf16 inputs (error budget = bf16 output rounding, 2^-8 relative).
@@ -127,6 +127,7 @@ def _attn_ref(qkv, lens, H, KV, hd):
     return out
 
 
+# the test names below keep the kernel generation they were written for; the kernel they check is attention_tc.cu
 @pytest.mark.parametrize("hd,H,KV", [(64, 3, 3), (64, 4, 2), (128, 2, 2), (128, 4, 1)])
 def test_attention_tcgen05_ragged_lengths_and_kernel_name(hd, H, KV):
     """Every tile-boundary case of the 128-row / 128-key tiling (and the 16-key granularity of the last tile), a
@@ -135,15 +136,15 @@ def test_attention_tcgen05_ragged_lengths_and_kernel_name(hd, H, KV):
     qkv = _rand(sum(lens), (H + 2 * KV) * hd, seed=7 * hd + H, scale=0.8)
     cu = torch.tensor(np.cumsum([0] + lens), dtype=torch.int32, device=DEV)
     got = enc.attention(qkv.to(DEV), cu, max(lens), H, KV, hd).float().cpu()
-    assert _lib.lib().ezr_attn_last_kernel() == b"tcgen05"
+    assert _lib.lib().ezr_attn_last_kernel() == b"wgmma"
     ref = _attn_ref(qkv, lens, H, KV, hd)
     _close(got.view(-1, H, hd), ref, rtol=2e-2, atol=1e-2)
 
 
 @pytest.mark.parametrize("hd", [64, 128])
 def test_attention_tcgen05_rescales_when_the_row_maximum_grows(hd):
-    """Keys are arranged so that every later key tile raises the row maximum by far more than 2^8: the lazy
-    rescaling of O in tensor memory must fire on every tile (and must not fire wrongly on flat tiles)."""
+    """Keys are arranged so that every later key tile raises the row maximum by far more than 2^8: the online
+    rescaling of O must be right on every tile (and on flat tiles)."""
     H = KV = 2
     lens = [640, 384, 130]
     t = sum(lens)
@@ -165,7 +166,7 @@ def test_attention_tcgen05_rescales_when_the_row_maximum_grows(hd):
 
 
 def test_attention_tcgen05_agrees_with_the_mma_sync_kernel():
-    """Two independent implementations of the same function (tcgen05 vs the warp-level kernel it replaced)."""
+    """Two independent implementations of the same function (wgmma vs the warp-level mma.sync kernel)."""
     L = _lib.lib()
     hd, H, KV = 64, 12, 12
     g = torch.Generator().manual_seed(5)

@@ -390,8 +390,11 @@ def _check_dense(res, c, qv, k, allowed=None, exact=False, id_base=0):
             assert m[got].all()
 
 
-# 1 = generic SIMT, 2 = tcgen05 (queries in smem), 3 = tcgen05 (queries in TMEM, 64-row tiles), 4 = same, 128-row tiles,
-# 5 = 4 in cluster pairs (each CTA loads half of every corpus tile and TMA-multicasts it to both)
+# 1 = generic SIMT, 2 = wgmma with 128-query blocks (dim <= 768), 3 = wgmma with 64-query blocks, 4 = same with 128-row
+# corpus tiles, 5 = 4 in cluster pairs (each CTA loads half of every corpus tile and TMA-multicasts it to both)
+KERNEL_NAMES = {1: b"simt", 2: b"wgmma", 3: b"wgmma-q64", 4: b"wgmma-q64-n128", 5: b"wgmma-q64-n128-mc2"}
+
+
 @pytest.mark.parametrize("kernel", [1, 2, 3, 4, 5])
 @pytest.mark.parametrize("n,d,q,k", [(5000, 128, 130, 10), (777, 768, 3, 5), (64, 64, 1, 16), (20_000, 768, 257, 10),
                                      (100, 256, 5, 12)])
@@ -401,20 +404,19 @@ def test_dense_exact_integer_inputs(kernel, n, d, q, k):
     _lib.check(L.ezr_dense_set_kernel(kernel))
     try:
         res = batched.dense_topk(DenseIndex(c, device=DEV), qv.to(DEV), k)
-        assert L.ezr_dense_last_kernel() == {1: b"simt", 2: b"tcgen05", 3: b"tcgen05-ts", 4: b"tcgen05-ts128",
-                                             5: b"tcgen05-ts128-mc2"}[kernel]
+        assert L.ezr_dense_last_kernel() == KERNEL_NAMES[kernel]
     finally:
         L.ezr_dense_set_kernel(0)
     _check_dense(res, c, qv, k, exact=True)
 
 
 def test_dense_wide_dims_cluster_pair_kernel():
-    c, qv = _dense_case(70_000, 1024, 300, 270, integer=True)      # odd number of query blocks (3), 1024-d, several splits
+    c, qv = _dense_case(70_000, 1024, 300, 270, integer=True)      # odd number of query blocks (5), 1024-d, several splits
     L = _lib.lib()
     _lib.check(L.ezr_dense_set_kernel(5))
     try:
         res = batched.dense_topk(DenseIndex(c, device=DEV), qv.to(DEV), 10)
-        assert L.ezr_dense_last_kernel() == b"tcgen05-ts128-mc2"
+        assert L.ezr_dense_last_kernel() == KERNEL_NAMES[5]
     finally:
         L.ezr_dense_set_kernel(0)
     _check_dense(res, c, qv, 10, exact=True)
@@ -422,24 +424,25 @@ def test_dense_wide_dims_cluster_pair_kernel():
 
 @pytest.mark.parametrize("n,d,q,k", [(3000, 1024, 130, 10), (2500, 832, 5, 8), (70_000, 1024, 300, 10)])
 def test_dense_wide_dims_use_hybrid_tmem_smem_queries(n, d, q, k):
-    # BGE-large is 1024-d (BASELINE config 5): part of the query block sits in TMEM (512 columns of it with
-    # 128-row tiles, 768 with 64-row tiles), the rest in shared memory
+    # BGE-large is 1024-d (BASELINE config 5): a 128-query block of that width does not fit shared memory beside the
+    # corpus ring, so the automatic choice is the 64-query block with 128-row corpus tiles; the 64-row-tile form is
+    # forced as well, and the 128-query form refuses the shape
     c, qv = _dense_case(n, d, q, 200 + n, integer=True)
     res = batched.dense_topk(DenseIndex(c, device=DEV), qv.to(DEV), k)
-    assert _lib.lib().ezr_dense_last_kernel() == b"tcgen05-ts128"
+    assert _lib.lib().ezr_dense_last_kernel() == KERNEL_NAMES[4]
     _check_dense(res, c, qv, k, exact=True)
     L = _lib.lib()
     _lib.check(L.ezr_dense_set_kernel(3))
     try:
         res = batched.dense_topk(DenseIndex(c, device=DEV), qv.to(DEV), k)
-        assert L.ezr_dense_last_kernel() == b"tcgen05-ts"
+        assert L.ezr_dense_last_kernel() == KERNEL_NAMES[3]
     finally:
         L.ezr_dense_set_kernel(0)
     _check_dense(res, c, qv, k, exact=True)
     _lib.check(L.ezr_dense_set_kernel(2))
     try:
         with pytest.raises(_lib.EzrError):
-            batched.dense_topk(DenseIndex(c, device=DEV), qv.to(DEV), k)      # SS variant stops at 768
+            batched.dense_topk(DenseIndex(c, device=DEV), qv.to(DEV), k)      # 128-query blocks stop at 768
     finally:
         L.ezr_dense_set_kernel(0)
 
