@@ -96,6 +96,15 @@ SIGNATURES = {
                                        C.POINTER(C.c_int64), _p]),
     "ezr_rerank_pack_fill": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p, _i32, _p, _i32, _i32, _i32,
                                        _p, _p, _p, _p]),
+    "ezr_cross_pack_workspace": (_sz, [_i32, _i32]),
+    "ezr_cross_pack_plan": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _i32, _i32, _p, _p,
+                                      C.POINTER(C.c_int64), _p, _sz, _p]),
+    "ezr_cross_pack_fill": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _i32, _i32, _i32, _i32,
+                                      _i32, _i32, _p, _p, _p, _p, _p]),
+    "ezr_cross_score_topk": (C.c_int, [_p, _i64, _p, _i32, _i32, _p, _i32, _p, C.c_float, _i32, _i32, _p, _p, _p, _p,
+                                       _p]),
+    "ezr_bert_embed_typed": (C.c_int, [_p, _p, _p, _i32, _p, _p, _p, _i32, _p, _p, C.c_float, _i32, _i32, _i32, _p,
+                                       _p]),
     "ezr_fuse_lists": (C.c_int, [_i32, _i32, _p, _p, _p, _i32, _i32, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
     "ezr_fusion_simple": (C.c_int, [_p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i32, _p, _p, _p, _p]),
 }

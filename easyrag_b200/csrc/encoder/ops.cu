@@ -52,9 +52,12 @@ __global__ void embed_gather_kernel(const int32_t* __restrict__ ids, const __nv_
 }
 
 // ------------------------------------------------- BERT embeddings: word + position + type, then LayerNorm
+// TYPED: token t adds row types[t] of the [n_types, dim] type table; otherwise every token adds row 0 (type_table).
+template <bool TYPED>
 __global__ void bert_embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ positions,
-                                     const __nv_bfloat16* __restrict__ word, const __nv_bfloat16* __restrict__ pos,
-                                     const __nv_bfloat16* __restrict__ type0, const __nv_bfloat16* __restrict__ gamma,
+                                     const int32_t* __restrict__ types, const __nv_bfloat16* __restrict__ word,
+                                     const __nv_bfloat16* __restrict__ pos, const __nv_bfloat16* __restrict__ type_table,
+                                     int n_types, const __nv_bfloat16* __restrict__ gamma,
                                      const __nv_bfloat16* __restrict__ beta, float eps, int vocab, int max_pos, int dim,
                                      __nv_bfloat16* __restrict__ out, int n_tokens) {
     extern __shared__ float sh_x[];          // dim floats + 33 scratch
@@ -65,10 +68,16 @@ __global__ void bert_embed_ln_kernel(const int32_t* __restrict__ ids, const int3
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
     int pp = positions[t];
     pp = pp < 0 ? 0 : (pp >= max_pos ? max_pos - 1 : pp);
+    const __nv_bfloat16* trow = type_table;
+    if (TYPED) {
+        int tt = types[t];
+        tt = tt < 0 ? 0 : (tt >= n_types ? n_types - 1 : tt);
+        trow += (int64_t)tt * dim;
+    }
     float s = 0.f;
     for (int i = threadIdx.x; i < dim; i += blockDim.x) {
         // each addend is a bf16 tensor in a bf16 model: word + type, then + position, each sum rounded (HF BertEmbeddings order)
-        float v = __bfloat162float(__float2bfloat16(__bfloat162float(word[(int64_t)id * dim + i]) + __bfloat162float(type0[i])));
+        float v = __bfloat162float(__float2bfloat16(__bfloat162float(word[(int64_t)id * dim + i]) + __bfloat162float(trow[i])));
         v = __bfloat162float(__float2bfloat16(v + __bfloat162float(pos[(int64_t)pp * dim + i])));
         sh_x[i] = v;
         s += v;
@@ -343,9 +352,25 @@ int ezr_bert_embed(const int32_t* ids, const int32_t* positions, int32_t n_token
     if (n_tokens == 0) return EZR_OK;
     EZR_CHECK_ARG(dim <= 8192, "bert_embed: dim too large");
     ProfScope prof(EZR_PROF_ENC_OTHER, (cudaStream_t)stream);
-    bert_embed_ln_kernel<<<n_tokens, norm_threads(dim), (dim + 40) * sizeof(float), (cudaStream_t)stream>>>(
-        ids, positions, (const __nv_bfloat16*)word, (const __nv_bfloat16*)pos, (const __nv_bfloat16*)type0,
+    bert_embed_ln_kernel<false><<<n_tokens, norm_threads(dim), (dim + 40) * sizeof(float), (cudaStream_t)stream>>>(
+        ids, positions, nullptr, (const __nv_bfloat16*)word, (const __nv_bfloat16*)pos, (const __nv_bfloat16*)type0, 1,
         (const __nv_bfloat16*)gamma, (const __nv_bfloat16*)beta, eps, vocab, max_pos, dim, (__nv_bfloat16*)out, n_tokens);
+    EZR_LAUNCH_CHECK();
+    return EZR_OK;
+}
+
+int ezr_bert_embed_typed(const int32_t* ids, const int32_t* positions, const int32_t* types, int32_t n_tokens,
+                         const void* word, const void* pos, const void* type_table, int32_t n_types, const void* gamma,
+                         const void* beta, float eps, int32_t vocab, int32_t max_pos, int32_t dim, void* out,
+                         void* stream) {
+    if (n_tokens == 0) return EZR_OK;
+    EZR_CHECK_ARG(dim <= 8192, "bert_embed_typed: dim too large");
+    EZR_CHECK_ARG(types && type_table && n_types >= 1, "bert_embed_typed: needs types and a type table of >= 1 row");
+    ProfScope prof(EZR_PROF_ENC_OTHER, (cudaStream_t)stream);
+    bert_embed_ln_kernel<true><<<n_tokens, norm_threads(dim), (dim + 40) * sizeof(float), (cudaStream_t)stream>>>(
+        ids, positions, types, (const __nv_bfloat16*)word, (const __nv_bfloat16*)pos, (const __nv_bfloat16*)type_table,
+        n_types, (const __nv_bfloat16*)gamma, (const __nv_bfloat16*)beta, eps, vocab, max_pos, dim, (__nv_bfloat16*)out,
+        n_tokens);
     EZR_LAUNCH_CHECK();
     return EZR_OK;
 }

@@ -131,11 +131,194 @@ static int fill_params(RerankParams& a, const int32_t* cand_ids, const int32_t* 
     return EZR_OK;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Cross-encoder pairs (SentenceTransformerRerank -> CrossEncoder.predict, rerankers.py:15-99): the fast tokenizer's
+// pair encoding with truncation="longest_first" at max_length, built from query and passage ids tokenised once
+// without special tokens.  Layout [cls] q' [sep] x n_mid p' [sep]; token type 0 up to the first [sep], type_b after;
+// positions pos_offset + i.  Only the real pairs are written (candidate r of query q with r < counts[q]), compacted in
+// query order: pair pair_off[q] + r.
+struct CrossParams {
+    const int32_t* cand_ids;    // [Q, k_stride] document ids in rank order
+    const int32_t* cand_cnt;    // [Q]
+    int n_queries, k, k_stride, id_base, n_docs;
+    const int32_t* q_ptr;       // [Q + 1] into q_tok
+    const int32_t* q_tok;
+    const int64_t* p_ptr;       // [n_docs + 1] into p_tok
+    const int32_t* p_tok;
+    int cls, sep, n_mid, type_b, pos_offset, max_length;
+};
+
+__device__ __forceinline__ int cross_count(const CrossParams& a, int q) { return min(max(a.cand_cnt[q], 0), a.k); }
+
+// the truncated lengths (a', b') of the tokenizer's longest_first rule with room T = max_length - specials
+__device__ __forceinline__ void cross_lengths(const CrossParams& a, int q, int doc, int& na, int& nb) {
+    const int64_t qa = a.q_ptr[q + 1] - a.q_ptr[q];
+    const int64_t pb = a.p_ptr[doc + 1] - a.p_ptr[doc];
+    const int64_t room = a.max_length - 2 - a.n_mid;
+    if (qa + pb <= room) { na = (int)qa; nb = (int)pb; }
+    else if (qa > pb) { nb = (int)min(pb, room / 2); na = (int)(room - nb); }
+    else { na = (int)min(qa, room / 2); nb = (int)(room - na); }
+}
+
+// per slot s = q * k + r: the pair length (0 for padding slots) and, once per query, the query's pair count.
+// A document id outside [id_base, id_base + n_docs) counts into *bad and gives an empty pair.
+__global__ void cross_len_kernel(const CrossParams a, int64_t* __restrict__ len, int64_t* __restrict__ n_pairs,
+                                 int32_t* __restrict__ bad) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= a.n_queries * a.k) return;
+    const int q = s / a.k, r = s % a.k;
+    const int n = cross_count(a, q);
+    if (r == 0) n_pairs[q] = n;
+    len[s] = 0;
+    if (r >= n) return;
+    const int doc = a.cand_ids[(int64_t)q * a.k_stride + r] - a.id_base;
+    if (doc < 0 || doc >= a.n_docs) { atomicAdd(bad, 1); return; }
+    int na, nb;
+    cross_lengths(a, q, doc, na, nb);
+    len[s] = 2 + a.n_mid + na + nb;
+}
+
+// pair_off (int32 [Q + 1]) and the compacted int32 cu [P + 1] from the two scans; slot_cu[Q * k] = T
+__global__ void cross_compact_kernel(const CrossParams a, const int64_t* __restrict__ slot_cu,
+                                     const int64_t* __restrict__ pair_off64, int32_t* __restrict__ pair_off,
+                                     int32_t* __restrict__ cu32, int64_t* __restrict__ totals) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n_slots = a.n_queries * a.k;
+    if (s > n_slots) return;
+    if (s == n_slots) {
+        cu32[pair_off64[a.n_queries]] = (int32_t)slot_cu[n_slots];
+        totals[0] = slot_cu[n_slots];
+        totals[1] = pair_off64[a.n_queries];
+        return;
+    }
+    const int q = s / a.k, r = s % a.k;
+    if (r == 0) pair_off[q] = (int32_t)pair_off64[q];
+    if (q == 0 && r == 0) pair_off[a.n_queries] = (int32_t)pair_off64[a.n_queries];
+    if (r < cross_count(a, q)) cu32[pair_off64[q] + r] = (int32_t)slot_cu[s];
+}
+
+// one warp per slot
+__global__ void cross_fill_kernel(const CrossParams a, const int64_t* __restrict__ slot_cu, int32_t* __restrict__ ids,
+                                  int32_t* __restrict__ types, int32_t* __restrict__ pos) {
+    const int s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (s >= a.n_queries * a.k) return;
+    const int64_t o = slot_cu[s], n = slot_cu[s + 1] - o;
+    if (n == 0) return;
+    const int q = s / a.k, r = s % a.k;
+    const int doc = a.cand_ids[(int64_t)q * a.k_stride + r] - a.id_base;
+    int na, nb;
+    cross_lengths(a, q, doc, na, nb);
+    const int32_t* qs = a.q_tok + a.q_ptr[q];
+    const int32_t* ps = a.p_tok + a.p_ptr[doc];
+    const int b0 = 1 + na + a.n_mid;                           // first passage token
+    for (int i = lane; i < n; i += 32) {
+        int t;
+        if (i == 0) t = a.cls;
+        else if (i <= na) t = qs[i - 1];
+        else if (i < b0) t = a.sep;
+        else if (i < b0 + nb) t = ps[i - b0];
+        else t = a.sep;
+        ids[o + i] = t;
+        types[o + i] = i <= na + 1 ? 0 : a.type_b;
+        pos[o + i] = a.pos_offset + i;
+    }
+}
+
+static int cross_params(CrossParams& a, const int32_t* cand_ids, const int32_t* cand_cnt, int n_queries, int k,
+                        int k_stride, int id_base, int n_docs, const int32_t* q_ptr, const int32_t* q_tok,
+                        const int64_t* p_ptr, const int32_t* p_tok, int cls, int sep, int n_mid, int type_b,
+                        int pos_offset, int max_length) {
+    EZR_CHECK_ARG(cand_ids && cand_cnt && q_ptr && p_ptr, "cross_pack: NULL argument");
+    EZR_CHECK_ARG(n_queries >= 0 && k >= 1 && k_stride >= k && n_docs >= 0, "cross_pack: bad n_queries / k / stride");
+    EZR_CHECK_ARG((int64_t)n_queries * k < ((int64_t)1 << 30), "cross_pack: too many pairs");
+    EZR_CHECK_ARG(n_mid == 1 || n_mid == 2, "cross_pack: n_mid must be 1 (BERT) or 2 (RoBERTa)");
+    EZR_CHECK_ARG(type_b == 0 || type_b == 1, "cross_pack: type_b must be 0 or 1");
+    EZR_CHECK_ARG(max_length >= 2 + n_mid && pos_offset >= 0, "cross_pack: max_length=%d leaves no room for the %d "
+                  "special tokens", max_length, 2 + n_mid);
+    a.cand_ids = cand_ids; a.cand_cnt = cand_cnt; a.n_queries = n_queries; a.k = k; a.k_stride = k_stride;
+    a.id_base = id_base; a.n_docs = n_docs; a.q_ptr = q_ptr; a.q_tok = q_tok; a.p_ptr = p_ptr; a.p_tok = p_tok;
+    a.cls = cls; a.sep = sep; a.n_mid = n_mid; a.type_b = type_b; a.pos_offset = pos_offset; a.max_length = max_length;
+    return EZR_OK;
+}
+
 }  // namespace ezr
 
 using namespace ezr;
 
 extern "C" {
+
+size_t ezr_cross_pack_workspace(int32_t n_queries, int32_t k) {
+    const size_t n_slots = (size_t)n_queries * k;
+    return align_up((2 * n_slots + 1) * 8, 256) + align_up(((size_t)2 * n_queries + 1) * 8, 256) + 256;
+}
+
+int ezr_cross_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k,
+                        int32_t k_stride, int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int64_t* p_ptr,
+                        int32_t n_mid, int32_t max_length, int32_t* out_pair_off, int32_t* out_cu,
+                        int64_t* totals_host, void* workspace, size_t ws_bytes, void* stream) {
+    CrossParams a;
+    int rc = cross_params(a, cand_ids, cand_cnt, n_queries, k, k_stride, id_base, n_docs, q_ptr, nullptr, p_ptr,
+                          nullptr, 0, 0, n_mid, 0, 0, max_length);
+    if (rc) return rc;
+    EZR_CHECK_ARG(out_pair_off && out_cu && totals_host, "cross_pack_plan: NULL output");
+    EZR_CHECK_ARG(workspace && ws_bytes >= ezr_cross_pack_workspace(n_queries, k), "cross_pack_plan: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int n_slots = n_queries * k;
+    if (n_queries == 0) {
+        totals_host[0] = totals_host[1] = 0;
+        EZR_CUDA(cudaMemsetAsync(out_pair_off, 0, 4, st));
+        EZR_CUDA(cudaMemsetAsync(out_cu, 0, 4, st));
+        return EZR_OK;
+    }
+    // workspace: len[n_slots] slot_cu[n_slots + 1] | n_pairs[Q] pair_off64[Q + 1] | totals[2] bad
+    char* w = static_cast<char*>(workspace);
+    int64_t* len = reinterpret_cast<int64_t*>(w);
+    int64_t* slot_cu = len + n_slots;
+    w += align_up((2 * (size_t)n_slots + 1) * 8, 256);
+    int64_t* n_pairs = reinterpret_cast<int64_t*>(w);
+    int64_t* pair_off64 = n_pairs + n_queries;
+    w += align_up(((size_t)2 * n_queries + 1) * 8, 256);
+    int64_t* totals = reinterpret_cast<int64_t*>(w);
+    int32_t* bad = reinterpret_cast<int32_t*>(totals + 2);
+    EZR_CUDA(cudaMemsetAsync(bad, 0, 4, st));
+    cross_len_kernel<<<ceil_div(n_slots, 256), 256, 0, st>>>(a, len, n_pairs, bad);
+    EZR_LAUNCH_CHECK();
+    rerank_scan_kernel<<<1, 1024, 0, st>>>(len, n_slots, slot_cu);
+    EZR_LAUNCH_CHECK();
+    rerank_scan_kernel<<<1, 1024, 0, st>>>(n_pairs, n_queries, pair_off64);
+    EZR_LAUNCH_CHECK();
+    cross_compact_kernel<<<ceil_div(n_slots + 1, 256), 256, 0, st>>>(a, slot_cu, pair_off64, out_pair_off, out_cu,
+                                                                       totals);
+    EZR_LAUNCH_CHECK();
+    int64_t h[3] = {0, 0, 0};
+    EZR_CUDA(cudaMemcpyAsync(h, totals, 16 + 4, cudaMemcpyDeviceToHost, st));
+    EZR_CUDA(cudaStreamSynchronize(st));
+    const int32_t n_bad = *reinterpret_cast<const int32_t*>(h + 2);
+    EZR_CHECK_ARG(n_bad == 0, "cross_pack_plan: %d candidate ids outside [id_base, id_base + n_docs) = [%d, %lld)", n_bad,
+                  id_base, (long long)id_base + n_docs);
+    totals_host[0] = h[0];
+    totals_host[1] = h[1];
+    return EZR_OK;
+}
+
+int ezr_cross_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k,
+                        int32_t k_stride, int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int32_t* q_tok,
+                        const int64_t* p_ptr, const int32_t* p_tok, int32_t cls, int32_t sep, int32_t n_mid,
+                        int32_t type_b, int32_t pos_offset, int32_t max_length, const void* workspace,
+                        int32_t* out_ids, int32_t* out_types, int32_t* out_pos, void* stream) {
+    CrossParams a;
+    int rc = cross_params(a, cand_ids, cand_cnt, n_queries, k, k_stride, id_base, n_docs, q_ptr, q_tok, p_ptr, p_tok,
+                          cls, sep, n_mid, type_b, pos_offset, max_length);
+    if (rc) return rc;
+    EZR_CHECK_ARG(q_tok && p_tok && workspace && out_ids && out_types && out_pos, "cross_pack_fill: NULL argument");
+    const int n_slots = n_queries * k;
+    if (n_slots == 0) return EZR_OK;
+    const int64_t* slot_cu = static_cast<const int64_t*>(workspace) + n_slots;
+    cross_fill_kernel<<<ceil_div(n_slots, 8), 256, 0, (cudaStream_t)stream>>>(a, slot_cu, out_ids, out_types, out_pos);
+    EZR_LAUNCH_CHECK();
+    return EZR_OK;
+}
 
 int ezr_rerank_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k, int32_t k_stride,
                          int32_t id_base, const int32_t* q_ptr, const int64_t* p_ptr, int32_t n_sep, int32_t n_prompt,

@@ -1,0 +1,87 @@
+// Cross-encoder head + per-query re-ordering (SentenceTransformerRerank._postprocess_nodes, rerankers.py:57-99).
+//
+// The head of BertForSequenceClassification / (XLM)RobertaForSequenceClassification with num_labels == 1 is
+//     CLS row -> Linear(d, d) + bias -> tanh -> Linear(d, 1) + bias -> sigmoid      (CrossEncoder.predict)
+// The CLS gather and the first Linear run as ezr_pool_normalize + ezr_gemm_bf16; this file is the rest, one CTA per
+// query: tanh, the d-wide dot with the output row, bias and sigmoid in fp32 for each of the query's pairs, then the
+// order of sorted(nodes, key=lambda x: -x.score if x.score else 0): score descending, ties in coarse-rank order
+// (a sigmoid is never negative, so a score of exactly 0 simply sorts last).  The order is taken on the fp32 sigmoid,
+// not on the logit: a trained reranker saturates many candidates to 1.0f, and the reference keeps their coarse order.
+#include "ezr_common.cuh"
+#include "../../include/easyrag_b200.h"
+
+namespace ezr {
+
+constexpr int kCrossThreads = 256;
+constexpr int kCrossMaxK = 1024;
+
+__device__ __forceinline__ float cross_warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+__global__ void __launch_bounds__(kCrossThreads)
+cross_score_topk_kernel(const __nv_bfloat16* __restrict__ dense, int64_t ldd, const int32_t* __restrict__ pair_off,
+                        int k, const int32_t* __restrict__ cand_ids, int k_stride, const float* __restrict__ w_out,
+                        float b_out, int dim, int top_n, float* __restrict__ out_all, float* __restrict__ out_scores,
+                        int32_t* __restrict__ out_ids, int32_t* __restrict__ out_counts) {
+    __shared__ float s_sc[kCrossMaxK];
+    const int q = blockIdx.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int p0 = pair_off[q];
+    const int n = min(pair_off[q + 1] - p0, k);
+    // one warp per pair; the lane-strided partial sums and the shuffle tree fix the summation order
+    for (int r = warp; r < n; r += kCrossThreads / 32) {
+        const __nv_bfloat16* row = dense + (int64_t)(p0 + r) * ldd;
+        float acc = 0.f;
+        for (int i = lane; i < dim; i += 32) acc = fmaf(tanhf(__bfloat162float(row[i])), w_out[i], acc);
+        acc = cross_warp_sum(acc);
+        if (lane == 0) s_sc[r] = 1.f / (1.f + expf(-(acc + b_out)));
+    }
+    __syncthreads();
+    for (int r = threadIdx.x; r < k; r += kCrossThreads) out_all[(int64_t)q * k + r] = r < n ? s_sc[r] : -INFINITY;
+    for (int r = threadIdx.x; r < n; r += kCrossThreads) {
+        const float sr = s_sc[r];
+        int pos = 0;
+        for (int j = 0; j < n; ++j) {
+            const float sj = s_sc[j];
+            pos += (sj > sr || (sj == sr && j < r)) ? 1 : 0;       // stable descending
+        }
+        if (pos < top_n) {
+            out_scores[(int64_t)q * top_n + pos] = sr;
+            out_ids[(int64_t)q * top_n + pos] = cand_ids[(int64_t)q * k_stride + r];
+        }
+    }
+    const int c = min(n, top_n);
+    for (int i = c + threadIdx.x; i < top_n; i += kCrossThreads) {
+        out_scores[(int64_t)q * top_n + i] = -INFINITY;
+        out_ids[(int64_t)q * top_n + i] = -1;
+    }
+    if (threadIdx.x == 0) out_counts[q] = c;
+}
+
+}  // namespace ezr
+
+using namespace ezr;
+
+extern "C" {
+
+int ezr_cross_score_topk(const void* dense, int64_t ldd, const int32_t* pair_off, int32_t n_queries, int32_t k,
+                         const int32_t* cand_ids, int32_t k_stride, const float* w_out, float b_out, int32_t dim,
+                         int32_t top_n, float* out_all, float* out_scores, int32_t* out_ids, int32_t* out_counts,
+                         void* stream) {
+    EZR_CHECK_ARG(n_queries >= 0 && k >= 1 && k <= kCrossMaxK && k_stride >= k,
+                  "cross_score_topk: k=%d out of [1, %d] (or k_stride < k)", k, kCrossMaxK);
+    EZR_CHECK_ARG(dim >= 1 && top_n >= 1, "cross_score_topk: dim and top_n must be >= 1");
+    EZR_CHECK_ARG(pair_off && cand_ids && w_out && out_all && out_scores && out_ids && out_counts,
+                  "cross_score_topk: NULL argument");
+    if (n_queries == 0) return EZR_OK;
+    cross_score_topk_kernel<<<n_queries, kCrossThreads, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16*)dense, ldd, pair_off, k, cand_ids, k_stride, w_out, b_out, dim, top_n, out_all,
+        out_scores, out_ids, out_counts);
+    EZR_LAUNCH_CHECK();
+    return EZR_OK;
+}
+
+}  // extern "C"

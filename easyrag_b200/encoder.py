@@ -92,6 +92,7 @@ class PackedBatch:
     max_len: int
     n_seq: int
     max_pos: Optional[int] = None   # largest position id + 1 (host-known when built by from_lists / from_padded)
+    types: Optional[torch.Tensor] = None   # int32 [T] token type ids (BERT-shaped encoders); None = type 0 everywhere
 
     def check_positions(self, limit: int) -> None:
         """The rope / position-embedding kernels index tables of ``limit`` rows; an id past the table would read
@@ -291,7 +292,8 @@ class BertEncoder:
         g = lambda name: state[name]
         self.word = _bf16(g("embeddings.word_embeddings.weight"), dev)
         self.pos = _bf16(g("embeddings.position_embeddings.weight"), dev)
-        self.type0 = _bf16(g("embeddings.token_type_embeddings.weight")[0], dev)
+        self.type_table = _bf16(g("embeddings.token_type_embeddings.weight"), dev)
+        self.type0 = self.type_table[0]
         self.emb_g = _bf16(g("embeddings.LayerNorm.weight"), dev)
         self.emb_b = _bf16(g("embeddings.LayerNorm.bias"), dev)
         self.layers = []
@@ -321,10 +323,17 @@ class BertEncoder:
         with torch.cuda.device(dev):
             st = _lib.stream_ptr()
             x = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
-            _lib.check(L.ezr_bert_embed(_lib.ptr(batch.ids), _lib.ptr(batch.positions), t, _lib.ptr(self.word),
-                                        _lib.ptr(self.pos), _lib.ptr(self.type0), _lib.ptr(self.emb_g),
-                                        _lib.ptr(self.emb_b), cfg.layer_norm_eps, cfg.vocab_size,
-                                        cfg.max_position_embeddings, d, _lib.ptr(x), st), "ezr_bert_embed")
+            if batch.types is None:
+                _lib.check(L.ezr_bert_embed(_lib.ptr(batch.ids), _lib.ptr(batch.positions), t, _lib.ptr(self.word),
+                                            _lib.ptr(self.pos), _lib.ptr(self.type0), _lib.ptr(self.emb_g),
+                                            _lib.ptr(self.emb_b), cfg.layer_norm_eps, cfg.vocab_size,
+                                            cfg.max_position_embeddings, d, _lib.ptr(x), st), "ezr_bert_embed")
+            else:
+                _lib.check(L.ezr_bert_embed_typed(_lib.ptr(batch.ids), _lib.ptr(batch.positions), _lib.ptr(batch.types),
+                                                  t, _lib.ptr(self.word), _lib.ptr(self.pos), _lib.ptr(self.type_table),
+                                                  self.type_table.shape[0], _lib.ptr(self.emb_g), _lib.ptr(self.emb_b),
+                                                  cfg.layer_norm_eps, cfg.vocab_size, cfg.max_position_embeddings, d,
+                                                  _lib.ptr(x), st), "ezr_bert_embed_typed")
             qkv = torch.empty(t, 3 * d, dtype=torch.bfloat16, device=dev)
             ao = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
             y = torch.empty(t, d, dtype=torch.bfloat16, device=dev)

@@ -11,6 +11,7 @@ from __future__ import annotations
 
 import asyncio
 import uuid
+from enum import Enum
 from typing import Any, Dict, List, Optional, Sequence, Union
 
 try:  # pragma: no cover - exercised only where llama_index is installed
@@ -158,6 +159,39 @@ except Exception:  # ModuleNotFoundError here
         async def aget_text_embedding_batch(self, texts: List[str], show_progress: bool = False, **kwargs: Any
                                             ) -> List[List[float]]:
             return self.get_text_embedding_batch(texts, show_progress=show_progress, **kwargs)
+
+
+# the node-postprocessor base of the rerankers (rerankers.py:6-7): its own fallback, since a llama_index install may
+# predate or omit the postprocessor module
+try:  # pragma: no cover - exercised only where llama_index is installed
+    from llama_index.core.postprocessor.types import BaseNodePostprocessor  # type: ignore
+    from llama_index.core.schema import MetadataMode  # type: ignore
+except Exception:
+    class MetadataMode(str, Enum):
+        ALL = "all"
+        EMBED = "embed"
+        LLM = "llm"
+        NONE = "none"
+
+    class BaseNodePostprocessor:
+        """postprocess_nodes wraps _postprocess_nodes; a bare query string becomes a QueryBundle."""
+
+        def __init__(self, callback_manager=None, **kwargs: Any) -> None:
+            self.callback_manager = callback_manager
+            for name, value in kwargs.items():        # the declared fields of a subclass (pydantic would validate them)
+                setattr(self, name, value)
+
+        def _postprocess_nodes(self, nodes: List[NodeWithScore],
+                               query_bundle: Optional[QueryBundle] = None) -> List[NodeWithScore]:
+            raise NotImplementedError
+
+        def postprocess_nodes(self, nodes: List[NodeWithScore], query_bundle: Optional[QueryBundle] = None,
+                              query_str: Optional[str] = None) -> List[NodeWithScore]:
+            if query_str is not None and query_bundle is not None:
+                raise ValueError("Cannot specify both query_str and query_bundle")
+            if query_str is not None:
+                query_bundle = QueryBundle(query_str)
+            return self._postprocess_nodes(nodes, query_bundle)
 
 
 class VectorStoreQuery:

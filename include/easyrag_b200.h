@@ -269,6 +269,38 @@ int ezr_rerank_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32
                          int32_t bos, int32_t max_length, const int64_t* cu, int32_t* out_ids, int32_t* out_cu32,
                          void* stream);
 
+/* ---------------------------------------------------- cross-encoder rerank ---
+ * SentenceTransformerRerank (rerankers.py:15-99): CrossEncoder.predict over (query, passage) pairs, then the stable
+ * descending sort of the sigmoid scores.  Pairs are built on the device from the coarse [Q, k] ids exactly as the
+ * fast tokenizer encodes a pair with truncation="longest_first" at max_length: with a, b the query / passage lengths
+ * (no specials) and T = max_length - 2 - n_mid, both stay if a + b <= T, else the longer side is cut to T - the other,
+ * where the other keeps min(its length, T/2); tokens are cut from the end.  Layout [cls] q [sep] x n_mid p [sep]
+ * (BERT n_mid = 1, types 0 | type_b = 1 after the first [sep]; RoBERTa / XLM-R n_mid = 2, type_b = 0), positions
+ * pos_offset + i (0 for BERT, padding_idx + 1 for RoBERTa).  Queries (q_ptr / q_tok) and passages (p_ptr / p_tok,
+ * n_docs of them, ids id_base ...) are device CSR arrays of ids tokenised without special tokens.
+ * Only the real pairs (candidate r < counts[q]) are packed: pair pair_off[q] + r, P = pair_off[Q] in all.
+ * plan: pair_off int32 [Q + 1], cu int32 [P + 1] (the caller sizes it Q * k + 1), totals_host = {T, P}
+ *       (synchronises; a candidate id outside the passage range is EZR_ERR_INVALID).
+ * fill: ids / types / positions int32 [T], reading the plan's workspace. */
+size_t ezr_cross_pack_workspace(int32_t n_queries, int32_t k);
+int ezr_cross_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k,
+                        int32_t k_stride, int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int64_t* p_ptr,
+                        int32_t n_mid, int32_t max_length, int32_t* out_pair_off, int32_t* out_cu,
+                        int64_t* totals_host, void* workspace, size_t ws_bytes, void* stream);
+int ezr_cross_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k,
+                        int32_t k_stride, int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int32_t* q_tok,
+                        const int64_t* p_ptr, const int32_t* p_tok, int32_t cls, int32_t sep, int32_t n_mid,
+                        int32_t type_b, int32_t pos_offset, int32_t max_length, const void* workspace,
+                        int32_t* out_ids, int32_t* out_types, int32_t* out_pos, void* stream);
+/* The rest of the head and the order, one CTA per query: dense = the [P, d] bf16 rows Linear(d, d) + bias made from
+ * the pairs' CLS rows; score = sigmoid(tanh(dense) . w_out + b_out) in fp32.  out_all [Q, k] holds every pair's
+ * score (-inf past the query's count); out_scores / out_ids [Q, top_n] the top_n by score descending, ties in coarse
+ * rank order (ids from cand_ids, -1 / -inf padded); out_counts [Q].  k <= 1024. */
+int ezr_cross_score_topk(const void* dense, int64_t ldd, const int32_t* pair_off, int32_t n_queries, int32_t k,
+                         const int32_t* cand_ids, int32_t k_stride, const float* w_out, float b_out, int32_t dim,
+                         int32_t top_n, float* out_all, float* out_scores, int32_t* out_ids, int32_t* out_counts,
+                         void* stream);
+
 /* ------------------------------------------------------------ encoder ---
  * Building blocks of the chunk/query embedding forward pass (GTEEmbedding._embed, gte_embeddings.py:59-72 ->
  * Qwen2Model.forward, modeling_qwen.py:956-1116; HuggingFaceEmbedding._embed, hf_embeddings.py:112-123 ->
@@ -297,6 +329,12 @@ int ezr_embed_gather(const int32_t* ids, int32_t n_tokens, const void* table, in
 int ezr_bert_embed(const int32_t* ids, const int32_t* positions, int32_t n_tokens, const void* word, const void* pos,
                    const void* type0, const void* gamma, const void* beta, float eps, int32_t vocab, int32_t max_pos,
                    int32_t dim, void* out, void* stream);
+/* the same with a per-token segment: LayerNorm(word[id] + type_table[types[t]] + position[pos]), n_types table rows
+ * (same rounding order: word + type, then + position, each rounded to bf16) */
+int ezr_bert_embed_typed(const int32_t* ids, const int32_t* positions, const int32_t* types, int32_t n_tokens,
+                         const void* word, const void* pos, const void* type_table, int32_t n_types, const void* gamma,
+                         const void* beta, float eps, int32_t vocab, int32_t max_pos, int32_t dim, void* out,
+                         void* stream);
 /* Qwen2RMSNorm (modeling_qwen.py:91-96) */
 int ezr_rmsnorm(const void* x, int64_t ldx, const void* gamma, float eps, int32_t n_rows, int32_t dim, void* out,
                 int64_t ldo, void* stream);
