@@ -198,7 +198,8 @@ int ezr_dense_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t
     }
     if (tc_ok && g_force_kernel != 1) {
         // auto (measured on one H100, 1M rows): 128-query blocks while they fit (dim <= 768) and the batch fills them
-        // (31.9 vs 34.9 ms for 10k queries at dim 768); otherwise 64-query blocks with 128-row corpus tiles
+        // (23.7 ms with query chunks in registers and 128-row tiles vs 34.9 ms for 64-query blocks, 10k queries at
+        // dim 768; 0.87 ms at 256 queries); otherwise 64-query blocks with 128-row corpus tiles
         // (dim 1024, 10k queries: 43.6 vs 60.4 ms for 64-row tiles; 64 queries at dim 768: 0.59 vs 0.68 ms)
         const bool wide_block = dense_tc_max_qw(dim) == 2 && n_queries > 64;
         const int form = g_force_kernel >= 2 ? g_force_kernel - 2 : (wide_block ? 0 : 2);

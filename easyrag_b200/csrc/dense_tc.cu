@@ -7,12 +7,13 @@
 //   for a long run of corpus rows (n_rows / n_splits), so the per-thread top-k lists warm up once per unit and almost
 //   nothing passes the threshold afterwards, and the query blocks resident at the same time stream the SAME corpus
 //   split, so a corpus tile is fetched from HBM once and served to the other CTAs from the L2.
-//   A query block (QW x 64 queries, QW = 2 consumer warpgroups for dim <= 768, 1 above) sits in shared memory for
-//   the whole unit (A operand, K-major, 128B-swizzled, 64 x 64 TMA boxes); the corpus rows stream through a ring of
-//   8 KB TMA stages (B operand: 64 rows x 64 bf16).  Each consumer warpgroup issues wgmma.m64n64k16 into 32 fp32
-//   registers per thread and scans its scores with a per-thread register-resident sorted list of k <= 16 per query
-//   row.  Scores never reach HBM: per (query, split) the four threads that share a query row write k (score, id)
-//   pairs each, and a warp-per-query merge produces the final list.
+//   A query block (QW x 64 queries, QW = 2 consumer warpgroups for dim <= 768, 1 above) stays resident for the whole
+//   unit (A operand; in shared memory as K-major, 128B-swizzled 64 x 64 TMA boxes, with the 128-query form holding
+//   its first k-chunks in registers instead); the corpus rows stream through a ring of TMA stages (B operand: TN rows
+//   x 64 bf16).  Each consumer warpgroup issues wgmma.m64nTNk16 into TN / 2 fp32 registers per thread and scans its
+//   scores with a per-thread register-resident sorted list of k <= 16 per query row.  Scores never reach HBM: per
+//   (query, split) the four threads that share a query row write k (score, id) pairs each, and a warp-per-query merge
+//   produces the final list.
 #include "ezr_common.cuh"
 #include "ptx.cuh"
 #include "dense_tc.h"
@@ -51,7 +52,14 @@ struct TcParams {
     int n_slices;
     int n_qblocks;        // units = n_slices x n_qblocks, walked by persistent CTAs
     int probe;            // measurement probes (ezr_dense_set_probe): 1 = no TMA loads, 2 = no MMAs, 4 = no epilogue scan; results are garbage
+    const __nv_bfloat16* queries;   // read directly (register-held query chunks of dense_wgmma_rq_kernel)
+    int64_t ldq;
 };
+
+// Query k-chunks the 128-query kernel holds in registers as wgmma A fragments (16 registers per thread each): the
+// most that fit beside 64 accumulators and the two top-k lists without spilling under the 232-register budget (lists of
+// 12 take 56 registers, of 16 take 72).
+__host__ __device__ constexpr int tc_reg_chunks(int kt) { return kt <= 8 ? 4 : kt == 12 ? 2 : 0; }
 
 struct TcBarriers {
     uint64_t a_full;       // the unit's query block has landed
@@ -313,6 +321,186 @@ dense_wgmma_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     if (CL > 1) ptx::cluster_sync();
 }
 
+// The 128-query form.  Warpgroup 0 = TMA producer (one thread, register budget lowered to 40), then two consumer
+// warpgroups (64 query rows each, raised to 232 registers).  A 9-warp CTA with a producer warp would not have more:
+// warps are spread over the SM's four register files, and the one holding three warps caps every thread at 168.
+// Each consumer keeps the first nreg = min(RQ, kchunks) k-chunks of its 64 query rows in registers as wgmma A
+// fragments, loaded once per unit from global memory (the query matrix stays in L2), and only the remaining chunks
+// sit in shared memory.  The freed space holds a deeper ring of 128-row corpus stages (16 KB).  Chunks below nreg
+// issue the register-A form (m64n128k16, B K-major), the others the shared-memory form; every score is still the
+// fp32 sum of the same k16 products in increasing k order.
+template <bool FILTER, int KT>
+__global__ void __launch_bounds__(384, 1)
+dense_wgmma_rq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
+                      const TcParams p) {
+    constexpr int RQ = tc_reg_chunks(KT);
+    constexpr int TN = 128;
+    constexpr int B_STAGE_BYTES = TN * TC_KC * 2;
+    extern __shared__ unsigned char smem_dyn[];
+    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    const int nreg = min(RQ, p.kchunks);
+    const int nsm = p.kchunks - nreg;                                         // query chunks in shared memory
+    unsigned char* smem_a = smem;                                             // [2][nsm] boxes of 8 KB
+    unsigned char* smem_b = smem + (size_t)2 * nsm * TC_A_BOX_BYTES;
+    TcBarriers* bars = reinterpret_cast<TcBarriers*>(smem_b + (size_t)p.n_stages * B_STAGE_BYTES);
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int n_units = p.n_slices * p.n_qblocks;
+
+    if (threadIdx.x == 0) {
+        ptx::prefetch_tensormap(&map_c);
+        ptx::prefetch_tensormap(&map_q);
+        ptx::mbar_init(&bars->a_full, 1);
+        ptx::mbar_init(&bars->a_empty, 2);
+        for (int i = 0; i < p.n_stages; ++i) {
+            ptx::mbar_init(&bars->b_full[i], 1);
+            ptx::mbar_init(&bars->b_empty[i], 2);
+        }
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        ptx::regs_dealloc<40>();
+        if (threadIdx.x == 0) {
+            // ---------------- TMA producer: shared-memory query chunks + corpus tiles of every unit, back to back
+            int stage = 0;
+            uint32_t phase = 0;
+            int ui = 0;
+            for (int u = blockIdx.x; u < n_units; u += gridDim.x, ++ui) {
+                const int slice = u / p.n_qblocks;
+                const int q0 = (u % p.n_qblocks) * 128;
+                const int64_t row_begin = (int64_t)slice * p.rows_per_slice;
+                const int64_t row_end = min(p.n_rows, row_begin + p.rows_per_slice);
+                const int n_tiles = (int)((row_end - row_begin + TN - 1) / TN);
+                ptx::mbar_wait(&bars->a_empty, ((uint32_t)ui & 1u) ^ 1u);    // the previous unit's MMAs are done
+                if (nsm == 0) {
+                    ptx::mbar_arrive(&bars->a_full);
+                } else {
+                    ptx::mbar_expect_tx(&bars->a_full, (uint32_t)(2 * nsm * TC_A_BOX_BYTES));
+                    for (int w = 0; w < 2; ++w)
+                        for (int kc = nreg; kc < p.kchunks; ++kc)
+                            ptx::tma_load_2d_hint(smem_a + (size_t)(w * nsm + kc - nreg) * TC_A_BOX_BYTES, &map_q,
+                                                  &bars->a_full, kc * TC_KC, q0 + w * 64, ptx::kEvictLast);
+                }
+                for (int t = 0; t < n_tiles; ++t) {
+                    const int row0 = (int)(row_begin + (int64_t)t * TN);
+                    for (int kc = 0; kc < p.kchunks; ++kc) {
+                        ptx::mbar_wait(&bars->b_empty[stage], phase ^ 1);
+                        if (p.probe & 1) {
+                            ptx::mbar_arrive(&bars->b_full[stage]);
+                        } else {
+                            ptx::mbar_expect_tx(&bars->b_full[stage], B_STAGE_BYTES);
+                            ptx::tma_load_2d(smem_b + (size_t)stage * B_STAGE_BYTES, &map_c, &bars->b_full[stage],
+                                             kc * TC_KC, row0);
+                        }
+                        if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
+                    }
+                }
+            }
+        }
+    } else {
+        // ---------------- consumers: warpgroup cw owns query rows [64 cw, 64 cw + 64) of the block
+        ptx::regs_alloc<232>();
+        const int cw = (threadIdx.x >> 7) - 1;
+        const int wq = warp & 3;
+        const bool leader = (threadIdx.x & 127) == 0;
+        const uint32_t a_base = ptx::smem_u32(smem_a) + (uint32_t)(cw * nsm * TC_A_BOX_BYTES);
+        const uint32_t b_base = ptx::smem_u32(smem_b);
+        int stage = 0;
+        uint32_t phase = 0;
+        int ui = 0;
+        for (int u = blockIdx.x; u < n_units; u += gridDim.x, ++ui) {
+            const int slice = u / p.n_qblocks;
+            const int q0 = (u % p.n_qblocks) * 128 + cw * 64;
+            const int64_t row_begin = (int64_t)slice * p.rows_per_slice;
+            const int64_t row_end = min(p.n_rows, row_begin + p.rows_per_slice);
+            const int n_tiles = (int)((row_end - row_begin + TN - 1) / TN);
+            const int qr = q0 + wq * 16 + (lane >> 2);        // accumulator fragment rows qr and qr + 8
+            RowList<KT> L0, L1;
+            row_start<KT>(L0, qr, p, FILTER);
+            row_start<KT>(L1, qr + 8, p, FILTER);
+            // A fragments of the register chunks (ptx.cuh, wgmma fragment layout); rows past n_queries are zero
+            uint32_t qa[RQ > 0 ? RQ : 1][4][4];
+            {
+                const unsigned int* r0 = reinterpret_cast<const unsigned int*>(p.queries + (int64_t)qr * p.ldq);
+                const unsigned int* r1 = reinterpret_cast<const unsigned int*>(p.queries + (int64_t)(qr + 8) * p.ldq);
+                const bool ok0 = qr < p.n_queries, ok1 = qr + 8 < p.n_queries;
+#pragma unroll
+                for (int kc = 0; kc < RQ; ++kc) {
+#pragma unroll
+                    for (int k4 = 0; k4 < 4; ++k4) {
+                        const int c = (kc * TC_KC + k4 * 16 + 2 * (lane & 3)) >> 1;     // bf16 pair index
+                        const bool in = kc < nreg;
+                        qa[kc][k4][0] = (in && ok0) ? __ldg(r0 + c) : 0u;
+                        qa[kc][k4][1] = (in && ok1) ? __ldg(r1 + c) : 0u;
+                        qa[kc][k4][2] = (in && ok0) ? __ldg(r0 + c + 4) : 0u;
+                        qa[kc][k4][3] = (in && ok1) ? __ldg(r1 + c + 4) : 0u;
+                    }
+                }
+            }
+            ptx::mbar_wait(&bars->a_full, (uint32_t)ui & 1u);
+
+            for (int t = 0; t < n_tiles; ++t) {
+                float acc[TN / 2];
+#pragma unroll
+                for (int i = 0; i < TN / 2; ++i) acc[i] = 0.f;
+                int prev = -1;
+                // the previous chunk's MMAs are done: hand its stage back to the producer
+                auto next_stage = [&]() {
+                    ptx::wgmma_wait<1>();
+                    if (prev >= 0 && leader) ptx::mbar_arrive(&bars->b_empty[prev]);
+                    prev = stage;
+                    if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
+                };
+#pragma unroll
+                for (int kc = 0; kc < RQ; ++kc) {
+                    if (kc < nreg) {
+                        ptx::mbar_wait(&bars->b_full[stage], phase);
+                        if (!(p.probe & 2) || kc == 0) {
+                            ptx::wgmma_fence();
+#pragma unroll
+                            for (int k4 = 0; k4 < TC_KC / 16; ++k4) {
+                                const uint64_t db = ptx::make_desc_sw128(b_base + (uint32_t)(stage * B_STAGE_BYTES + k4 * 32));
+                                ptx::wgmma_rs_n128(acc, qa[kc][k4], db, (uint32_t)((kc | k4) != 0));
+                            }
+                            ptx::wgmma_commit();
+                        }
+                        next_stage();
+                    }
+                }
+                for (int kc = nreg; kc < p.kchunks; ++kc) {
+                    ptx::mbar_wait(&bars->b_full[stage], phase);
+                    if (!(p.probe & 2)) {
+                        ptx::wgmma_fence();
+#pragma unroll
+                        for (int k4 = 0; k4 < TC_KC / 16; ++k4) {
+                            const uint64_t da = ptx::make_desc_sw128(a_base + (uint32_t)((kc - nreg) * TC_A_BOX_BYTES + k4 * 32));
+                            const uint64_t db = ptx::make_desc_sw128(b_base + (uint32_t)(stage * B_STAGE_BYTES + k4 * 32));
+                            ptx::wgmma_ss_n128(acc, da, db, 1u);
+                        }
+                        ptx::wgmma_commit();
+                    }
+                    next_stage();
+                }
+                ptx::wgmma_wait<0>();
+                ptx::fence_regs(acc);
+                if (leader) {
+                    ptx::mbar_arrive(&bars->b_empty[prev]);
+                    if (t == n_tiles - 1) ptx::mbar_arrive(&bars->a_empty);    // the unit's last read of the query block
+                }
+                // ---- epilogue: this thread's 32 scores of each of its two rows
+                const int64_t doc0 = row_begin + (int64_t)t * TN + (lane & 3) * 2;
+                scan_row<FILTER, KT, 0, TN>(acc, L0, doc0, row_end - doc0, p);
+                scan_row<FILTER, KT, 1, TN>(acc, L1, doc0, row_end - doc0, p);
+            }
+            row_finish<KT>(L0, slice, lane & 3, p);
+            row_finish<KT>(L1, slice, lane & 3, p);
+        }
+    }
+}
+
 // ------------------------------------------------------------------ host ----
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -396,7 +584,7 @@ int dense_tc_max_qw(int dim) { return dim <= 768 ? 2 : 1; }
 
 // kernel forms: (query blocks of 64 * QW rows, corpus tiles of TN rows, CTAs per cluster)
 struct TcForm { int qw, tn, cl; const char* name; };
-static const TcForm kForms[4] = {{2, 64, 1, "wgmma"}, {1, 64, 1, "wgmma-q64"}, {1, 128, 1, "wgmma-q64-n128"},
+static const TcForm kForms[4] = {{2, 128, 1, "wgmma"}, {1, 64, 1, "wgmma-q64"}, {1, 128, 1, "wgmma-q64-n128"},
                                  {1, 128, 2, "wgmma-q64-n128-mc2"}};
 
 const char* dense_tc_form_name(int form) { return kForms[form].name; }
@@ -436,7 +624,12 @@ int dense_tc_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t 
     p.doc_group = doc_group;
     p.q_group = q_group;
     p.probe = g_dense_probe;
-    const size_t a_bytes = (size_t)f.qw * p.kchunks * TC_A_BOX_BYTES;
+    p.queries = queries;
+    p.ldq = ldq;
+    const int kt = (k + 3) / 4 - 1;
+    // form 0 (dense_wgmma_rq_kernel) holds the first query chunks in registers; the rest sit in shared memory
+    const int reg_chunks = form == 0 ? min(tc_reg_chunks(4 * (kt + 1)), p.kchunks) : 0;
+    const size_t a_bytes = (size_t)f.qw * (p.kchunks - reg_chunks) * TC_A_BOX_BYTES;
     const size_t b_stage = (size_t)f.tn * TC_KC * 2;
     const size_t fixed = 1024 /*alignment slack*/ + sizeof(TcBarriers);
     int stages = (int)((TC_SMEM_LIMIT - fixed - a_bytes) / b_stage);
@@ -469,10 +662,13 @@ int dense_tc_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t 
       dense_wgmma_kernel<false, 12, QW, TN, CL>, dense_wgmma_kernel<false, 16, QW, TN, CL>},                        \
      {dense_wgmma_kernel<true, 4, QW, TN, CL>, dense_wgmma_kernel<true, 8, QW, TN, CL>,                             \
       dense_wgmma_kernel<true, 12, QW, TN, CL>, dense_wgmma_kernel<true, 16, QW, TN, CL>}}
-    static const kern_t table[4][2][4] = {EZR_DENSE_FORM(2, 64, 1), EZR_DENSE_FORM(1, 64, 1), EZR_DENSE_FORM(1, 128, 1),
-                                          EZR_DENSE_FORM(1, 128, 2)};
+    static const kern_t table[4][2][4] = {
+        {{dense_wgmma_rq_kernel<false, 4>, dense_wgmma_rq_kernel<false, 8>, dense_wgmma_rq_kernel<false, 12>,
+          dense_wgmma_rq_kernel<false, 16>},
+         {dense_wgmma_rq_kernel<true, 4>, dense_wgmma_rq_kernel<true, 8>, dense_wgmma_rq_kernel<true, 12>,
+          dense_wgmma_rq_kernel<true, 16>}},
+        EZR_DENSE_FORM(1, 64, 1), EZR_DENSE_FORM(1, 128, 1), EZR_DENSE_FORM(1, 128, 2)};
 #undef EZR_DENSE_FORM
-    const int kt = (k + 3) / 4 - 1;
     kern_t kern = table[form][fi][kt];
     static bool attr_done[4][2][4] = {};
     if (!attr_done[form][fi][kt]) {
