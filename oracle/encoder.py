@@ -34,21 +34,23 @@ def _rotate_half(x):
 
 
 def qwen2_hidden(state: Dict[str, torch.Tensor], cfg, input_ids: torch.Tensor, attention_mask: torch.Tensor,
-                 dtype=torch.float32) -> torch.Tensor:
-    """[B, L] ids + mask -> last_hidden_state [B, L, d] (final norm applied), non-causal, additive padding mask."""
+                 dtype=torch.float32, device="cpu") -> torch.Tensor:
+    """[B, L] ids + mask -> last_hidden_state [B, L, d] (final norm applied), non-causal, additive padding mask.
+    Runs on ``device``: weights, inputs and the position / mask / rotary tensors are all placed there."""
     d, H, KV = cfg.hidden_size, cfg.num_attention_heads, cfg.num_key_value_heads
     hd = d // H
-    w = {k: v.to(dtype) for k, v in state.items()}
+    w = {k: v.to(device=device, dtype=dtype) for k, v in state.items()}
+    input_ids, attention_mask = input_ids.to(device), attention_mask.to(device)
     b, l = input_ids.shape
     x = F.embedding(input_ids.long(), w["embed_tokens.weight"])
-    pos = torch.arange(l)
-    inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.int64).float() / hd))
+    pos = torch.arange(l, device=device)
+    inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.int64, device=device).float() / hd))
     freqs = torch.outer(pos.float(), inv_freq)
     emb = torch.cat((freqs, freqs), dim=-1)
     cos, sin = emb.cos().to(dtype)[None, None], emb.sin().to(dtype)[None, None]
     # padding-only additive mask (modeling_qwen.py:1052-1056 with is_causal=False)
     neg = torch.finfo(dtype).min
-    add = torch.zeros(b, 1, l, l, dtype=dtype)
+    add = torch.zeros(b, 1, l, l, dtype=dtype, device=device)
     add = add.masked_fill(attention_mask[:, None, None, :] == 0, neg)
     for i in range(cfg.num_hidden_layers):
         p = f"layers.{i}."
@@ -82,10 +84,10 @@ def last_token_pool(h: torch.Tensor, attention_mask: torch.Tensor) -> torch.Tens
     return h[torch.arange(h.shape[0]), lens]
 
 
-def gte_embed(state, cfg, input_ids, attention_mask, dtype=torch.float32) -> torch.Tensor:
-    """GTEEmbedding._embed after tokenisation (gte_embeddings.py:65-71) -> float32 [B, d]."""
-    h = qwen2_hidden(state, cfg, input_ids, attention_mask, dtype)
-    e = F.normalize(last_token_pool(h, attention_mask), p=2, dim=1)
+def gte_embed(state, cfg, input_ids, attention_mask, dtype=torch.float32, device="cpu") -> torch.Tensor:
+    """GTEEmbedding._embed after tokenisation (gte_embeddings.py:65-71) -> float32 [B, d] on ``device``."""
+    h = qwen2_hidden(state, cfg, input_ids, attention_mask, dtype, device)
+    e = F.normalize(last_token_pool(h, attention_mask.to(device)), p=2, dim=1)
     return e.to(torch.float)
 
 
