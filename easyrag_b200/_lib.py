@@ -103,6 +103,8 @@ SIGNATURES = {
                                       _i32, _i32, _p, _p, _p, _p, _p]),
     "ezr_cross_score_topk": (C.c_int, [_p, _i64, _p, _i32, _i32, _p, _i32, _p, C.c_float, _i32, _i32, _p, _p, _p, _p,
                                        _p]),
+    "ezr_cross_pair_scores": (C.c_int, [_p, _i32, _i32, _p, C.c_float, _p, _p]),
+    "ezr_cross_order_topk": (C.c_int, [_p, _p, _i32, _i32, _p, _i32, _i32, _p, _p, _p, _p, _p]),
     "ezr_bert_embed_typed": (C.c_int, [_p, _p, _p, _i32, _p, _p, _p, _i32, _p, _p, C.c_float, _i32, _i32, _i32, _p,
                                        _p]),
     "ezr_fuse_lists": (C.c_int, [_i32, _i32, _p, _p, _p, _i32, _i32, _p, _i32, _i32, _i32, _p, _p, _p, _p]),

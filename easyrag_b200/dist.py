@@ -1,4 +1,4 @@
-"""Row-sharded coarse ranking across the GPUs of one box (SURVEY.md section 8(e)).
+"""Row-sharded coarse ranking (SURVEY.md section 8(e)) and pair-split fine ranking across the GPUs of one box.
 
 The reference is single-process; this is new.  Corpus rows (and the BM25 document axis) are cut
 into contiguous shards, one per rank; queries are replicated.  Corpus-global BM25 statistics
@@ -8,12 +8,17 @@ SINGLE all-gather (NCCL over NVLink on GPUs, gloo in the CPU tests) exchanges th
 every rank then merges G*k candidates per route under the canonical order -- the same order
 the 1-GPU path uses, hence identical rank lists -- reading the gathered buffer in place, and
 runs RRF.
+
+Fine ranking (:class:`ShardedCrossEncoderReranker`) splits the other way: every rank holds the whole cross-encoder and
+the same candidate lists, the (query, candidate) pairs are cut into token-balanced runs, one per rank, and ONE
+all-reduce of a [P] fp32 score vector gives every rank every pair's score; each rank then orders all queries.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Optional, Tuple
+from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -163,3 +168,116 @@ class ShardedCoarseRanker:
 
     def join(self) -> None:
         self.ranker.join()
+
+
+def token_balanced_ranges(cu_h: Sequence[int], world: int) -> List[Tuple[int, int]]:
+    """Contiguous, ordered, exhaustive runs ``[lo, hi)`` of whole pairs, one per rank, with about equal token counts.
+
+    ``cu_h`` int [P + 1] holds the pairs' token offsets (T = ``cu_h[-1]``).  Rank r's run starts at the first pair whose
+    start token is >= r T / world, so a run holds less than T / world tokens plus the length of its last pair.  A run is
+    empty when P < world or when a long pair spans a whole share."""
+    if world < 1:
+        raise ValueError(f"world={world} must be >= 1")
+    cu = np.asarray(cu_h, dtype=np.int64)
+    n, t = cu.size - 1, int(cu[-1])
+    starts = cu[:-1] * world                          # start * world >= r * T  <=>  start >= r * T / world, exactly
+    bounds = [int(np.searchsorted(starts, r * t, side="left")) for r in range(world)] + [n]
+    return [(bounds[r], bounds[r + 1]) for r in range(world)]
+
+
+def exchange_pair_scores(sig: torch.Tensor, group=None) -> torch.Tensor:
+    """In place: each rank's ``sig`` float32 [P] holds the scores of its own run of pairs and +0.0 everywhere else;
+    afterwards every rank holds all P scores, bit for bit.
+
+    One ``all_reduce(SUM)``.  It is exact in any reduction order: every element has at most one contribution that is not
+    +0.0, a sigmoid is never negative (an underflow gives +0.0, never -0.0), and x + (+0.0) == x for every x >= +0.0.
+    Compared with an all-gather it needs no padding to the longest run and no copy into place afterwards: the scoring
+    kernel writes straight into the buffer that is reduced.  The message is 4 bytes per pair either way."""
+    dist.all_reduce(sig, op=dist.ReduceOp.SUM, group=group)
+    return sig
+
+
+def check_replicated(values: Sequence[int], what: str, group=None, device="cpu") -> None:
+    """Raise ``ValueError`` on every rank unless every rank passed the same ``values`` (one small all-gather)."""
+    world = dist.get_world_size(group)
+    mine = torch.tensor(list(values), dtype=torch.int64, device=device)
+    every = torch.empty(world * mine.numel(), dtype=torch.int64, device=device)
+    dist.all_gather_into_tensor(every, mine, group=group)
+    rows = every.view(world, -1).cpu()
+    if not bool((rows == rows[0]).all()):
+        raise ValueError(f"{what} differ across ranks (one row per rank): {rows.tolist()}; every rank must pass "
+                         f"the same input")
+
+
+class ShardedCrossEncoderReranker:
+    """:class:`easyrag_b200.rerank.CrossEncoderReranker` with the pairs split across ranks; every rank returns the full
+    result, bit-identical to one GPU's.
+
+    Every rank packs all pairs (deterministic and cheap, and it gives every rank the pairs' token offsets), then encodes
+    only its run of them (:func:`token_balanced_ranges`): the chunked encoder, the CLS rows, Linear + bias and the
+    per-pair sigmoid (``ezr_cross_pair_scores``) into its slice of a zeroed [P] fp32 buffer.  One
+    :func:`exchange_pair_scores` per batch completes the buffer and every rank orders all queries
+    (``ezr_cross_order_topk``).  A pair's score does not depend on the encoder pass it is in, hence the bit-identity.
+
+    ``cand``, ``q_ptr`` and ``q_tok`` must be the same on every rank (``ShardedCoarseRanker``'s output is); the
+    candidate shape and the pair and token totals are compared across ranks with one small all-gather per call.  With
+    no process group, or a group of one, this is the wrapped reranker on one GPU.
+    """
+
+    def __init__(self, reranker, group=None):
+        """``reranker``: a :class:`easyrag_b200.rerank.CrossEncoderReranker` on this rank's device (same model and
+        passages on every rank)."""
+        self.reranker = reranker
+        self.group = group
+        self.distributed = dist.is_available() and dist.is_initialized()
+        self.world = dist.get_world_size(group) if self.distributed else 1
+        self.rank = dist.get_rank(group) if self.distributed else 0
+        nccl = self.distributed and dist.get_backend(group) == dist.Backend.NCCL
+        self._check_device = reranker.device if nccl else "cpu"
+
+    def rerank(self, cand, q_ptr: torch.Tensor, q_tok: torch.Tensor, top_n: int,
+               events: Optional[List[torch.cuda.Event]] = None):
+        """Same arguments and results as ``CrossEncoderReranker.rerank``.  The stage events bracket: packing and the
+        cross-rank input check; this rank's encoder run; its head, the score exchange (which waits for the slowest
+        rank) and the order."""
+        from . import _lib
+        from .batched import TopK
+        from .encoder import gemm
+        from .rerank import MAX_CANDIDATES, _mark
+        L = _lib.lib()
+        rr = self.reranker
+        m, dev = rr.model, rr.device
+        if cand.ids.dim() == 2 and cand.ids.shape[1] > MAX_CANDIDATES:
+            raise ValueError(f"k={cand.ids.shape[1]} candidates per query; at most {MAX_CANDIDATES} are supported")
+        if top_n < 1:
+            raise ValueError("top_n must be >= 1")
+        _mark(events)
+        pairs = rr.pack(cand.ids, cand.counts, q_ptr, q_tok)
+        nq, k, n_pairs, d = pairs.n_queries, pairs.k, pairs.n_pairs, m.cfg.hidden_size
+        if self.distributed:
+            check_replicated((nq, k, n_pairs, int(pairs.cu_h[-1])), "candidate shape [Q, k], pair and token totals",
+                             self.group, self._check_device)
+        _mark(events)
+        lo, hi = token_balanced_ranges(pairs.cu_h, self.world)[self.rank]
+        out = TopK(torch.empty(nq, top_n, dtype=torch.float32, device=dev),
+                   torch.empty(nq, top_n, dtype=torch.int32, device=dev), torch.empty(nq, dtype=torch.int32, device=dev))
+        all_scores = torch.empty(nq, k, dtype=torch.float32, device=dev)
+        sig = torch.zeros(n_pairs, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            if hi > lo:
+                cls = torch.empty(hi - lo, d, dtype=torch.bfloat16, device=dev)
+                for p0, p1 in rr.chunks(pairs.cu_h[lo:hi + 1]):
+                    rr._encode_cls(pairs, lo + p0, lo + p1, cls[p0:p1])
+            _mark(events)
+            if hi > lo:
+                dense = gemm(cls, m.w1, bias=m.b1)
+                _lib.check(L.ezr_cross_pair_scores(_lib.ptr(dense), d, hi - lo, _lib.ptr(m.w2), m.b2,
+                                                   _lib.ptr(sig[lo:hi]), _lib.stream_ptr()), "ezr_cross_pair_scores")
+            if self.distributed and n_pairs:
+                exchange_pair_scores(sig, self.group)
+            _lib.check(L.ezr_cross_order_topk(_lib.ptr(sig), _lib.ptr(pairs.pair_off), nq, k, _lib.ptr(pairs.cand_ids),
+                                              pairs.cand_ids.stride(0), top_n, _lib.ptr(all_scores),
+                                              _lib.ptr(out.scores), _lib.ptr(out.ids), _lib.ptr(out.counts),
+                                              _lib.stream_ptr()), "ezr_cross_order_topk")
+            _mark(events)
+        return out, all_scores

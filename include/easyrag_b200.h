@@ -300,6 +300,16 @@ int ezr_cross_score_topk(const void* dense, int64_t ldd, const int32_t* pair_off
                          const int32_t* cand_ids, int32_t k_stride, const float* w_out, float b_out, int32_t dim,
                          int32_t top_n, float* out_all, float* out_scores, int32_t* out_ids, int32_t* out_counts,
                          void* stream);
+/* ezr_cross_score_topk in two steps, bit-identical to it, for pairs scored on several devices.
+ * pair_scores: out_sig[p] = sigmoid(tanh(dense[p]) . w_out + b_out) for the n_pairs contiguous [n_pairs, dim] bf16
+ *              rows of dense (one warp per pair).
+ * order_topk:  from sig float32 [P] (pair pair_off[q] + r = candidate r of query q), the outputs of
+ *              ezr_cross_score_topk (one CTA per query).  k <= 1024. */
+int ezr_cross_pair_scores(const void* dense, int32_t dim, int32_t n_pairs, const float* w_out, float b_out,
+                          float* out_sig, void* stream);
+int ezr_cross_order_topk(const float* sig, const int32_t* pair_off, int32_t n_queries, int32_t k,
+                         const int32_t* cand_ids, int32_t k_stride, int32_t top_n, float* out_all, float* out_scores,
+                         int32_t* out_ids, int32_t* out_counts, void* stream);
 
 /* ------------------------------------------------------------ encoder ---
  * Building blocks of the chunk/query embedding forward pass (GTEEmbedding._embed, gte_embeddings.py:59-72 ->
