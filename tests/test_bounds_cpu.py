@@ -1,8 +1,10 @@
-"""CPU: the bf16 error-bound checker of tests/_bounds.py accepts correct roundings and rejects biased or wrong ones."""
+"""CPU: the bf16 error-bound checker of tests/_bounds.py accepts correct roundings and rejects biased or wrong ones;
+the cross-encoder head's bound holds for an fp32 emulation of the kernel and rejects wrong references."""
 import pytest
 import torch
 
-from _bounds import check_bf16, rejects, round_bf16, ulp_bf16
+from _bounds import (Z_ONE, Z_SUB, Z_ZERO, check_bf16, check_sigmoid, cross_head_bound, cross_head_case,
+                     cross_head_logit, rejects, round_bf16, ulp_bf16, ulp_f32)
 
 N = 200_000
 
@@ -81,3 +83,104 @@ def test_preconditions():
         check_bf16(round_bf16(y).to(torch.bfloat16), y, 10 * ulp_bf16(y), "loose", median_ulps=2.0)
     with pytest.raises(AssertionError):
         rejects(check_bf16, round_bf16(y).to(torch.bfloat16), y, 10 * ulp_bf16(y), "loose", median_ulps=2.0)
+
+
+# ------------------------------------------------------------------------------------- cross-encoder head
+HEAD_PAIRS = 6000
+HEAD_MEDIAN_ULPS = 128     # the same figure the GPU test holds the bound to (tests/test_gpu_bert_shapes.py)
+
+
+def _ulps_off(exact, k):
+    """An fp32 result within 2 ulp of ``exact`` (fp64), as tanhf / expf guarantee: the nearest fp32 value moved by
+    ``k`` ulps, or left nearest where that would leave the 2-ulp band."""
+    near = exact.float()
+    u = ulp_f32(exact)
+    cand = (near.double() + k * u).float()
+    ok = (cand.double() - exact).abs() <= 2 * u
+    return torch.where(ok, cand, near)
+
+
+def _emulate_head(rows, w, b, k_tanh, k_exp):
+    """csrc/rerank.cu cross_pair_sigmoid in fp32 on the CPU, in the kernel's order: lane i % 32 accumulates element i
+    with fmaf, then the xor-shuffle tree adds the lanes.  fmaf is emulated as the fp64 value of t * w + acc (the
+    product is exact there) rounded to fp32: a double rounding, at most 2^-29 relative away from fmaf's one."""
+    t = _ulps_off(torch.tanh(rows.double()), k_tanh).clamp(-1, 1).double()
+    n, d = rows.shape
+    wd = w.double()
+    acc = torch.zeros(n, 32, dtype=torch.float32)
+    for i0 in range(0, d, 32):
+        m = min(32, d - i0)
+        acc[:, :m] = (t[:, i0:i0 + m] * wd[i0:i0 + m] + acc[:, :m].double()).float()
+    lane = torch.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        acc = acc + acc[:, lane ^ o]
+    z = acc[:, 0] + torch.tensor(b, dtype=torch.float32)
+    e = _ulps_off(torch.exp(-z.double()), k_exp)              # +inf past FLT_MAX
+    one = torch.ones((), dtype=torch.float32)
+    return one / (one + e)
+
+
+@pytest.fixture(scope="module", params=[768, 1000], ids=["d768", "d1000-ragged-lanes"])
+def head(request):
+    d = request.param
+    rows, w, b = cross_head_case(HEAD_PAIRS, d, 90 + d)
+    z, s, ds = cross_head_bound(rows, w, b)
+    return rows, w, b, z, s, ds
+
+
+def test_head_case_fills_every_band(head):
+    *_, z, _, _ = head
+    for lo, hi in ((-1, 1), (Z_ONE, 40), (Z_SUB[0], Z_SUB[1]), (-120, Z_ZERO)):
+        share = ((z > lo) & (z < hi)).double().mean().item()
+        assert share > 0.15, (lo, hi, share)
+
+
+def test_head_bound_holds_for_the_emulated_kernel(head):
+    rows, w, b, z, s, ds = head
+    g = torch.Generator().manual_seed(5)
+    k_t = torch.randint(-2, 3, rows.shape, generator=g)
+    k_e = torch.randint(-2, 3, (rows.shape[0],), generator=g)
+    got = _emulate_head(rows, w, b, k_t, k_e)
+    info = check_sigmoid(got, z, s, ds, "emulated head", median_ulps=HEAD_MEDIAN_ULPS, min_elems=HEAD_PAIRS)
+    # worst case within the functions' accuracy: every tanhf 2 ulp towards sign(w) (all push z up), expf 2 ulp down
+    sw = torch.sign(w).long()[None, :].expand(rows.shape)
+    up = _emulate_head(rows, w, b, 2 * sw, torch.full((rows.shape[0],), -2))
+    info_up = check_sigmoid(up, z, s, ds, "emulated head, errors aligned", median_ulps=HEAD_MEDIAN_ULPS,
+                            min_elems=HEAD_PAIRS, max_bias=1.0)
+    print(f"\n[bounds] head emulation: random {info}; aligned {info_up}")
+    assert info_up["bias"] > info["bias"]                    # the aligned errors show in the mean
+
+
+@pytest.mark.parametrize("control", ["bias dropped", "tanh rounded to bf16", "tanh omitted", "w_out shifted by one"])
+def test_head_bound_rejects_wrong_references(head, control):
+    rows, w, b, z, s, ds = head
+    got = _emulate_head(rows, w, b, torch.zeros(rows.shape, dtype=torch.long),
+                        torch.zeros(rows.shape[0], dtype=torch.long))
+    if control == "bias dropped":
+        zw = cross_head_logit(rows, w, 0.0)
+    elif control == "tanh rounded to bf16":
+        zw = cross_head_logit(rows, w, b, tanh=lambda x: round_bf16(torch.tanh(x)))
+    elif control == "tanh omitted":
+        zw = cross_head_logit(rows, w, b, tanh=lambda x: x)
+    else:
+        zw = cross_head_logit(rows, torch.roll(w, 1), b)
+    assert rejects(check_sigmoid, got, zw, torch.sigmoid(zw), ds, control, median_ulps=HEAD_MEDIAN_ULPS,
+                   min_elems=HEAD_PAIRS)
+
+
+def test_head_bound_preconditions(head):
+    rows, w, b, z, s, ds = head
+    got = _emulate_head(rows, w, b, torch.zeros(rows.shape, dtype=torch.long),
+                        torch.zeros(rows.shape[0], dtype=torch.long))
+    with pytest.raises(AssertionError, match="vacuous"):
+        check_sigmoid(got, z, s, 1e3 * ds, "loose", median_ulps=HEAD_MEDIAN_ULPS, min_elems=HEAD_PAIRS)
+    with pytest.raises(AssertionError, match="too few"):
+        check_sigmoid(got[:10], z[:10], s[:10], ds[:10], "small", median_ulps=HEAD_MEDIAN_ULPS)
+    sub = (z > Z_SUB[0]) & (z < Z_SUB[1])
+    flushed = torch.where(sub, torch.zeros_like(got), got)
+    with pytest.raises(AssertionError, match="flushed"):                 # a bound wide enough to pass zeros there
+        check_sigmoid(flushed, z, s, torch.where(sub, 2 * s, ds), "ftz", median_ulps=HEAD_MEDIAN_ULPS,
+                      min_elems=HEAD_PAIRS, max_bias=1.0)
+    neg0 = torch.where(z < Z_ZERO, torch.full_like(got, -0.0), got)
+    with pytest.raises(AssertionError, match=r"\+0\.0"):
+        check_sigmoid(neg0, z, s, ds, "-0", median_ulps=HEAD_MEDIAN_ULPS, min_elems=HEAD_PAIRS)

@@ -15,7 +15,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from _bounds import U32, check_bf16, rejects, round_bf16, ulp_bf16
+from _bounds import U32, check_bf16, ln_exact_and_delta, rejects, round_bf16, ulp_bf16
 from oracle import encoder as oenc
 from oracle import retrieve as ort
 from easyrag_b200 import _lib, batched, encoder as enc, synth
@@ -200,29 +200,6 @@ def _rms_exact(x, gamma, eps):
     return gamma.double() * round_bf16(X * rstd)
 
 
-def _ln_exact_and_delta(x, gamma, beta, eps):
-    """LayerNorm in fp64 and the bound on the kernel's fp32 error before its one bf16 rounding (ops.cu norm kernels:
-    two-pass mean / variance)."""
-    dim = x.shape[1]
-    X, G, B = x.double(), gamma.double(), beta.double()
-    mu = X.mean(-1, keepdim=True)
-    d = X - mu
-    var = d.pow(2).mean(-1, keepdim=True)
-    r = torch.rsqrt(var + eps)
-    exact = d * r * G + B
-    chain = dim / 32 + 10                 # longest fp32 addition chain of a row sum: dim / 32 serial adds per lane
-                                          # (dim / 128 in the block kernel) + 5 shuffle levels (+ 5 block levels)
-    e_mu = (chain + 1) * U32 * X.abs().mean(-1, keepdim=True)    # the row sum, then the division by dim
-    e_var = ((chain + 3) * U32                                   # sum of squares (+ square, division, eps add)
-             + 2 * e_mu * d.abs().mean(-1, keepdim=True) / var   # each d carries the mean's error
-             + e_mu ** 2 / var)
-    e_r = 0.5 * e_var + 2.0 ** -22 + U32                         # sqrt halves it; rsqrtf <= 2 ulp; the eps add
-    delta = (G.abs() * r * (e_mu + U32 * d.abs())                # x - mean: the mean's error, then its rounding
-             + (G * d * r).abs() * (e_r + 2 * U32)               # rstd's error; (d * rstd) * gamma rounded twice
-             + U32 * ((G * d * r).abs() + B.abs()))              # + beta rounded
-    return exact, delta
-
-
 RMS_CASES = [  # (dim, row stride): warp kernel MAXC = 16 (1032..4096), MAXC = 4 (<= 1024); block kernel otherwise
     (3584, None), (1536, None), (4096, None), (1032, None), (1024, None), (5120, None), (3588, None), (3584, 3587)]
 
@@ -254,7 +231,7 @@ def test_layernorm_model_dims(dim, eps, ld):
     gamma = (1 + 0.1 * torch.randn(dim, generator=_gen(18 + dim), device=DEV)).to(torch.bfloat16)
     beta = _randn(dim, seed=19 + dim, std=0.1)
     got = enc.layernorm(x, gamma, beta, eps)
-    exact, delta = _ln_exact_and_delta(x, gamma, beta, eps)
+    exact, delta = ln_exact_and_delta(x, gamma, beta, eps)
     info = check_bf16(got, exact, delta, f"layernorm {dim}", median_ulps=0.1)
     _report(f"layernorm dim={dim} eps={eps} ld={ld or dim}", info)
     # control: a one-pass variance E[x^2] - E[x]^2 accumulated serially in fp32 (what the offset rows defeat)
