@@ -8,8 +8,9 @@ unbiased (a kernel that truncates instead of rounding to nearest shows a mean si
 
 ``ln_exact_and_delta`` is the fp64 LayerNorm and the bound of the norm kernels' fp32 error.  ``cross_head_bound`` /
 ``check_sigmoid`` do the same for the cross-encoder head (csrc/rerank.cu), whose result is an fp32 sigmoid rather
-than a bf16 rounding.  Used by tests/test_gpu_model_shapes.py and tests/test_gpu_bert_shapes.py; checked itself by
-tests/test_bounds_cpu.py.
+than a bf16 rounding.  ``dense_score_bound`` / ``check_dense_topk`` bound the fp32 scores of the wgmma dense top-k
+(csrc/dense_tc.cu) and check its result lists against an fp64 top list.  Used by tests/test_gpu_model_shapes.py,
+tests/test_gpu_bert_shapes.py and tests/test_gpu_dense_scale.py; checked itself by tests/test_bounds_cpu.py.
 """
 import math
 
@@ -229,3 +230,113 @@ def cross_head_case(n_pairs: int, dim: int, seed: int, device="cpu"):
     x[:, ~steer] = xs.double()
     x[:, steer] = xv
     return x.to(torch.bfloat16), w, b
+
+
+# ------------------------------------------------------------------------------------------ dense top-k
+# The wgmma dense kernels (csrc/dense_tc.cu) compute each score as an fp32 accumulation over d / 16 k16 steps of
+# bf16 x bf16 products, which are exact in fp32.  How the tensor core adds the 16 products of a step to the
+# accumulator is not documented for Hopper: the products are aligned to the largest exponent and the sum may be
+# truncated rather than rounded.  Each step is therefore allowed 17 units of 2^-23 relative to |S_j| + sum |p_i|
+# (16 aligned products and the accumulator, each losing up to one ulp, plus the truncated result), where S_j is
+# the exact partial sum after step j.  Not fitted to a measurement: the ratio an H100 shows is reported, not used.
+DENSE_STEP_ULPS = 17
+DENSE_K = 16                     # products per wgmma k step (bf16)
+
+
+def dense_score_bound(q: torch.Tensor, c: torch.Tensor, ids: torch.Tensor, chunk: int = 1024):
+    """-> (exact, delta) [Q, k] fp64: the score of each (query, returned id) pair and the bound on the kernel's fp32
+    error in it.  ``q`` [Q, d], ``c`` [n, d] bf16 on one device; ``ids`` [Q, k] row indices (>= 0)."""
+    nq, d = q.shape
+    assert d % DENSE_K == 0
+    k = ids.shape[1]
+    exact = torch.empty(nq, k, dtype=torch.float64, device=q.device)
+    delta = torch.empty_like(exact)
+    for q0 in range(0, nq, chunk):
+        qq = q[q0:q0 + chunk].double()
+        rows = c[ids[q0:q0 + chunk].long()].double()                   # [Qc, k, d]
+        p = qq[:, None, :] * rows                                       # exact: 8 + 8 significant bits
+        steps = p.view(p.shape[0], k, d // DENSE_K, DENSE_K)
+        part = steps.sum(-1).cumsum(-1)                                 # S_j after each k16 step
+        exact[q0:q0 + chunk] = part[..., -1]
+        delta[q0:q0 + chunk] = DENSE_STEP_ULPS * 2.0 ** -23 * (part.abs().sum(-1) + p.abs().sum(-1))
+    return exact, delta
+
+
+def dense_delta_max(q: torch.Tensor, c_norm_max: float):
+    """[Q] fp64: an upper bound of ``dense_score_bound`` over every row of a corpus whose largest row norm is
+    ``c_norm_max``: |S_j| <= ||q|| ||c|| for each of the d / 16 steps, and sum |p_i| <= ||q|| ||c|| (Cauchy-Schwarz)."""
+    d = q.shape[1]
+    return DENSE_STEP_ULPS * 2.0 ** -23 * (d / DENSE_K + 1) * q.double().norm(dim=1) * c_norm_max
+
+
+def check_dense_topk(scores, ids, exact, delta, top_vals, top_ids, dmax, n_rows, what) -> dict:
+    """Assert that a top-k result (``scores`` fp32 / ``ids`` [Q, k], every query with k results) is the fp64 top-k up
+    to the kernel's error.  ``exact`` / ``delta``: fp64 score of each returned id and its bound (dense_score_bound);
+    ``top_vals`` / ``top_ids`` [Q, K > k]: the fp64 top list, descending; ``dmax`` [Q]: dense_delta_max.
+      * every returned score lies within delta of its id's fp64 score;
+      * every id whose fp64 score beats the fp64 k-th by more than 2 dmax is returned (nothing clearly better left out);
+      * no returned id scores below the fp64 k-th - 2 dmax;
+      * ids are distinct rows, scores non-increasing, equal scores ordered by id descending.
+    Returns the measured figures: worst |err| / delta, the share of scores equal to the fp32 rounding of the fp64
+    score, and the queries whose fp64 (k+1)-th lies within 2 dmax of the k-th (where either id may be returned)."""
+    nq, k = ids.shape
+    dev = exact.device
+    scores, ids = scores.to(dev), ids.to(dev).long()
+    top_vals, top_ids, dmax = top_vals.to(dev), top_ids.to(dev).long(), dmax.to(dev)
+    assert top_ids.shape[1] > k
+    assert ((ids >= 0) & (ids < n_rows)).all(), f"{what}: ids outside [0, {n_rows})"
+    srt = ids.sort(1).values
+    assert (srt[:, 1:] != srt[:, :-1]).all(), f"{what}: a row returned twice"
+    g = scores.double()
+    ratio = (g - exact).abs() / delta
+    w = int(torch.argmax(ratio))
+    wq, wj = divmod(w, k)
+    assert ratio.max() <= 1, (f"{what}: worst element query {wq} rank {wj} (id {int(ids[wq, wj])}): got "
+                              f"{g[wq, wj].item():.9g}, fp64 {exact[wq, wj].item():.9g}, bound "
+                              f"{delta[wq, wj].item():.3g}")
+    kth = top_vals[:, k - 1]
+    margin = 2 * dmax
+    must = top_vals[:, :k] > (kth + margin)[:, None]
+    found = (top_ids[:, :k, None] == ids[:, None, :]).any(-1)
+    miss = must & ~found
+    if miss.any():
+        mq, mj = (int(x) for x in torch.nonzero(miss)[0])
+        raise AssertionError(f"{what}: worst element query {mq}: id {int(top_ids[mq, mj])} (fp64 {top_vals[mq, mj].item():.9g}"
+                             f", rank {mj}) beats the k-th ({kth[mq].item():.9g}) by more than {margin[mq].item():.3g} "
+                             f"and is not returned")
+    low = exact < (kth - margin)[:, None]
+    if low.any():
+        lq, lj = (int(x) for x in torch.nonzero(low)[0])
+        raise AssertionError(f"{what}: worst element query {lq}: returned id {int(ids[lq, lj])} scores "
+                             f"{exact[lq, lj].item():.9g} in fp64, below the k-th {kth[lq].item():.9g} - {margin[lq].item():.3g}")
+    ds, di = scores[:, 1:] - scores[:, :-1], ids[:, 1:] - ids[:, :-1]
+    bad = (ds > 0) | ((ds == 0) & (di > 0))
+    assert not bad.any(), f"{what}: query {int(torch.nonzero(bad)[0, 0])}: not in (score desc, id desc) order"
+    return dict(worst=ratio.max().item(), rn_share=(g == exact.float().double()).double().mean().item(),
+                ambiguous=int((top_vals[:, k] >= kth - margin).sum()), queries=nq,
+                median_delta=delta.median().item(), median_dmax=dmax.median().item())
+
+
+# ------------------------------------------------------------------------------------------ L2 normalisation
+# normalize_rows_kernel (csrc/dense.cu), one warp per row, fp32 without fast-math:
+#     q   = sum of x_i^2: lane i % 32 runs ceil(d / 32) fmaf steps, then 5 xor-shuffle adds
+#     inv = 1.0f / fmaxf(sqrtf(q), 1e-12f)      (sqrtf and the division are IEEE, correctly rounded)
+#     out = bf16(x_i * inv)
+NORM_FLOOR = float(torch.tensor(1e-12, dtype=torch.float32))    # the fp32 value of 1e-12f
+
+
+def l2_normalize_exact_and_delta(x):
+    """-> (exact, delta): the fp64 value of the kernel's function (rows below the 1e-12f floor are scaled by
+    1 / 1e-12f, not normalised) and the bound on its fp32 error before the bf16 rounding.  Rows within a few ulps
+    of the floor are not covered (either branch may be taken there)."""
+    X = x.double()
+    nrm = X.norm(dim=1, keepdim=True)
+    exact = X / nrm.clamp_min(NORM_FLOOR)
+    steps = -(-x.shape[1] // 32)
+    rel = torch.where(nrm >= NORM_FLOOR,
+                      (steps + 5) * U32 / 2          # q: every fmaf / shuffle add rounds relative to a partial sum
+                                                     # <= q, so |q err| <= (steps + 5) u q; sqrt halves it
+                      + U32                          # sqrtf
+                      + 2 * U32,                     # 1 / norm; x * inv
+                      torch.full_like(nrm, 2 * U32))   # below the floor: 1 / 1e-12f and x * inv
+    return exact, exact.abs() * rel * (1 + 2.0 ** -10)   # the factor covers second-order terms

@@ -1,10 +1,13 @@
 """CPU: the bf16 error-bound checker of tests/_bounds.py accepts correct roundings and rejects biased or wrong ones;
-the cross-encoder head's bound holds for an fp32 emulation of the kernel and rejects wrong references."""
+the cross-encoder head's bound holds for an fp32 emulation of the kernel and rejects wrong references; the dense
+top-k score bound holds for an emulated truncating k16 accumulator, stays tight, and the membership check built on
+it rejects a wrong reference and a result that leaves out a clearly better row."""
 import pytest
 import torch
 
-from _bounds import (Z_ONE, Z_SUB, Z_ZERO, check_bf16, check_sigmoid, cross_head_bound, cross_head_case,
-                     cross_head_logit, rejects, round_bf16, ulp_bf16, ulp_f32)
+from _bounds import (Z_ONE, Z_SUB, Z_ZERO, check_bf16, check_dense_topk, check_sigmoid, cross_head_bound,
+                     cross_head_case, cross_head_logit, dense_delta_max, dense_score_bound, rejects, round_bf16,
+                     ulp_bf16, ulp_f32)
 
 N = 200_000
 
@@ -184,3 +187,98 @@ def test_head_bound_preconditions(head):
     neg0 = torch.where(z < Z_ZERO, torch.full_like(got, -0.0), got)
     with pytest.raises(AssertionError, match=r"\+0\.0"):
         check_sigmoid(neg0, z, s, ds, "-0", median_ulps=HEAD_MEDIAN_ULPS, min_elems=HEAD_PAIRS)
+
+
+# --------------------------------------------------------------------------------------------- dense top-k
+DENSE_ROWS, DENSE_DIM, DENSE_Q, DENSE_KEEP, DENSE_TOPK = 20_000, 768, 64, 64, 10
+DENSE_MEDIAN_ULPS = 1024     # median bound of a returned score, in fp32 ulps of the score (the GPU test's 1e-3
+                             # tolerance it replaces is ~17000 ulps at 0.5)
+
+
+def _to_f32(x, mode):
+    """fp64 -> fp32 rounded to nearest ("rn") or toward zero ("rz"), as fp64."""
+    r = x.float().double()
+    if mode == "rz":
+        over = r.abs() > x.abs()
+        r = torch.where(over, torch.nextafter(r.float(), torch.zeros_like(r.float())).double(), r)
+    return r
+
+
+def _emulate_dense(q, rows, mode):
+    """fp32 accumulation over k16 steps of the exact products of q [Q, d] with rows [Q, m, d]: each step adds its 16
+    products (summed exactly) to the accumulator and rounds the result to fp32 (``mode``)."""
+    p = q.double()[:, None, :] * rows.double()
+    steps = p.view(*p.shape[:2], -1, 16).sum(-1)
+    acc = torch.zeros(p.shape[:2], dtype=torch.float64)
+    for j in range(steps.shape[-1]):
+        acc = _to_f32(acc + steps[..., j], mode)
+    return acc
+
+
+@pytest.fixture(scope="module")
+def dense():
+    from easyrag_b200 import synth
+    c = synth.make_dense_corpus(DENSE_ROWS, DENSE_DIM, 61)
+    q = synth.make_dense_queries(c, DENSE_Q, 62)
+    sims = q.double() @ c.double().T
+    top_vals, top_ids = sims.topk(DENSE_KEEP, dim=1)
+    # the emulated kernel's top-k, among the fp64 top 64 (its errors are far below the gaps that far down)
+    emu = _emulate_dense(q, c[top_ids], "rz")
+    order = torch.argsort(top_ids, dim=1, descending=True)                 # id desc, then a stable sort by score
+    emu_s, emu_i = emu.gather(1, order), top_ids.gather(1, order)
+    order = torch.argsort(emu_s, dim=1, descending=True, stable=True)[:, :DENSE_TOPK]
+    got_s, got_i = emu_s.gather(1, order).float(), emu_i.gather(1, order)
+    exact, delta = dense_score_bound(q, c, got_i)
+    dmax = dense_delta_max(q, c.double().norm(dim=1).max().item())
+    return dict(c=c, q=q, top_vals=top_vals, top_ids=top_ids, got_s=got_s, got_i=got_i, exact=exact, delta=delta,
+                dmax=dmax)
+
+
+@pytest.mark.parametrize("mode", ["rz", "rn"])
+def test_dense_bound_holds_for_emulated_accumulator(dense, mode):
+    c, q, ids = dense["c"], dense["q"], dense["top_ids"]
+    emu = _emulate_dense(q, c[ids], mode)
+    exact, delta = dense_score_bound(q, c, ids)
+    ratio = ((emu - exact).abs() / delta).max().item()
+    print(f"\n[bounds] dense emulation ({mode}): worst |err| / delta = {ratio:.4g}")
+    assert ratio <= 1
+    assert (delta <= dense_delta_max(q, c.double().norm(dim=1).max().item())[:, None]).all()
+
+
+def test_dense_bound_is_not_vacuous(dense):
+    med = (dense["delta"] / ulp_f32(dense["exact"])).median().item()
+    print(f"\n[bounds] dense: median delta = {med:.4g} fp32 ulps, median delta max = "
+          f"{dense['dmax'].median().item():.3g}")
+    assert med <= DENSE_MEDIAN_ULPS
+    assert dense["dmax"].max().item() < 2e-4                 # unit vectors, d 768: 17 * 2^-23 * 49
+
+
+def _check(d, **over):
+    a = dict(d, **over)
+    return check_dense_topk(a["got_s"], a["got_i"], a["exact"], a["delta"], a["top_vals"], a["top_ids"], a["dmax"],
+                            DENSE_ROWS, "emulated dense")
+
+
+def test_dense_membership_accepts_emulated_and_rejects_controls(dense):
+    info = _check(dense)
+    print(f"\n[bounds] dense membership: {info}")
+    assert info["worst"] <= 1
+    c, q, k = dense["c"], dense["q"], DENSE_TOPK
+    # (a) a reference without the last 16 dims
+    cs, qs = c[:, :-16], q[:, :-16]
+    tv, ti = (qs.double() @ cs.double().T).topk(DENSE_KEEP, dim=1)
+    ex = (qs.double()[:, None, :] * cs[dense["got_i"]].double()).sum(-1)
+    assert rejects(_check, dense, top_vals=tv, top_ids=ti, exact=ex)
+    # (b) the best id of one query replaced by the fp64 (k+1)-th, its score the fp32 rounding of its fp64 score
+    tv, ti = dense["top_vals"], dense["top_ids"]
+    sep = (tv[:, 0] - tv[:, k - 1] > 2 * dense["dmax"]) & ~(ti[:, k:k + 1] == dense["got_i"]).any(1)
+    qi = int(torch.nonzero(sep)[0])
+    gi, gs, ge, gd = (dense[n].clone() for n in ("got_i", "got_s", "exact", "delta"))
+    j = int((gi[qi] == ti[qi, 0]).nonzero()[0])
+    gi[qi, j], gs[qi, j], ge[qi, j] = ti[qi, k], tv[qi, k].float(), tv[qi, k]
+    order = torch.argsort(gi[qi], descending=True)
+    order = order[torch.argsort(gs[qi][order], descending=True, stable=True)]
+    gi[qi], gs[qi], ge[qi], gd[qi] = gi[qi][order], gs[qi][order], ge[qi][order], gd[qi][order]
+    with pytest.raises(AssertionError, match="not returned"):
+        _check(dense, got_i=gi, got_s=gs, exact=ge, delta=gd)
+    assert rejects(_check, dense, got_i=gi, got_s=gs, exact=ge, delta=gd)

@@ -16,6 +16,7 @@ import torch
 import torch.nn.functional as F
 
 from _bounds import U32, check_bf16, ln_exact_and_delta, rejects, round_bf16, ulp_bf16
+from _topk_ref import canonical_topk
 from oracle import encoder as oenc
 from oracle import retrieve as ort
 from easyrag_b200 import _lib, batched, encoder as enc, synth
@@ -468,16 +469,6 @@ def int_case():
     return c, q, sims
 
 
-def _canonical_topk(sims, k, allowed=None):
-    """(score desc, id desc) top-k of exact integer scores: one int64 key per (score, id)."""
-    n = sims.shape[1]
-    key = sims.long() * (1 << 17) + torch.arange(n, device=DEV)
-    if allowed is not None:
-        key = torch.where(allowed, key, torch.full_like(key, torch.iinfo(torch.int64).min))
-    top = key.topk(k, dim=1).indices
-    return top, sims.gather(1, top)
-
-
 def _dense(index, q, k, q_group=None):
     res = batched.dense_topk(index, q, k, q_group=q_group)
     torch.cuda.synchronize()
@@ -489,7 +480,7 @@ def _dense(index, q, k, q_group=None):
 def test_dense_3584_exact_integers_bit_exact(int_case, k):
     c, q, sims = int_case
     res = _dense(DenseIndex(c, device=DEV), q, k)
-    ids, sc = _canonical_topk(sims, k)
+    ids, sc = canonical_topk(sims, k)
     assert (res.counts == k).all()
     assert torch.equal(res.ids.long(), ids)
     assert torch.equal(res.scores, sc.float())
@@ -508,7 +499,7 @@ def test_dense_3584_group_filter_with_row_lo(int_case):
     want[want == 4] = -2                                              # a class no row has: empty result
     res = _dense(DenseIndex(c, device=DEV, doc_group=groups, row_lo=lo), q, k, q_group=want)
     allowed = (want[:, None] == -1) | (groups[None, :] == want[:, None])
-    ids, sc = _canonical_topk(sims, k, allowed)
+    ids, sc = canonical_topk(sims, k, allowed)
     cnt = allowed.sum(1).clamp(max=k)
     assert torch.equal(res.counts.long(), cnt)
     assert (cnt == 0).any() and (cnt == k).any()
