@@ -44,8 +44,12 @@ class TopK:
 
 def dense_topk(index: DenseIndex, queries: torch.Tensor, k: int, q_group: Optional[torch.Tensor] = None,
                id_base: Optional[int] = None, ws: Optional[Workspace] = None, stream=None,
-               out: Optional[TopK] = None) -> TopK:
-    """QdrantRetriever._aretrieve's search for a batch (retrievers.py:37-52): cosine top-k, ids descending on ties."""
+               out: Optional[TopK] = None, cand_counts: Optional[torch.Tensor] = None) -> TopK:
+    """QdrantRetriever._aretrieve's search for a batch (retrievers.py:37-52): cosine top-k, ids descending on ties.
+
+    A quantized index runs ``ezr_dense_s8_topk`` (int8 candidate pass + exact rescoring; its scores are the
+    fixed-order fp32 ``rescore`` of csrc/dense_s8.cu).  ``cand_counts`` (int32 [Q] on the device, quantized indexes
+    only) receives the candidates per query of the int8 pass."""
     L = _lib.lib()
     dev = index.device
     q = queries
@@ -60,11 +64,22 @@ def dense_topk(index: DenseIndex, queries: torch.Tensor, k: int, q_group: Option
     if out is None:
         out = TopK(torch.empty(nq, k, dtype=torch.float32, device=dev), torch.empty(nq, k, dtype=torch.int32, device=dev),
                    torch.empty(nq, dtype=torch.int32, device=dev))
-    need = L.ezr_dense_topk_workspace(index.n_rows, dim, nq, k)
+    quantized = getattr(index, "quantized", False)
+    if cand_counts is not None and not quantized:
+        raise ValueError("cand_counts needs a quantized index")
+    need = (L.ezr_dense_s8_topk_workspace if quantized else L.ezr_dense_topk_workspace)(index.n_rows, dim, nq, k)
     ws = ws or Workspace(dev)
     buf = ws.get(need)
     base = index.row_lo if id_base is None else id_base
     with torch.cuda.device(dev):
+        if quantized:
+            _lib.check(L.ezr_dense_s8_topk(
+                _lib.ptr(index.vectors), index.n_rows, dim, index.vectors.stride(0), _lib.ptr(q), nq, q.stride(0), k,
+                _lib.ptr(index.doc_group if qg is not None else None), _lib.ptr(qg), base, _lib.ptr(out.scores),
+                _lib.ptr(out.ids), _lib.ptr(out.counts), _lib.ptr(index.rows_s8), index.rows_s8.stride(0),
+                _lib.ptr(index.row_scale), _lib.ptr(index.maxima), _lib.ptr(cand_counts), _lib.ptr(buf), buf.numel(),
+                _lib.stream_ptr(stream)), "ezr_dense_s8_topk")
+            return out
         _lib.check(L.ezr_dense_topk(_lib.ptr(index.vectors), index.n_rows, dim, index.vectors.stride(0), _lib.ptr(q), nq,
                                     q.stride(0), k, _lib.ptr(index.doc_group if qg is not None else None), _lib.ptr(qg),
                                     base, _lib.ptr(out.scores), _lib.ptr(out.ids), _lib.ptr(out.counts), _lib.ptr(buf),

@@ -16,6 +16,8 @@ namespace ezr {
 constexpr int kSimtTile = 64;
 constexpr int kSimtK = 32;
 
+// SEP: separate __fmul_rn / __fadd_rn (the rescore arithmetic of dense_s8.cu) instead of fmaf
+template <bool SEP>
 __global__ void __launch_bounds__(256)
 dense_scores_simt_kernel(const __nv_bfloat16* __restrict__ corpus, int64_t n_rows, int dim, int64_t ldc,
                          const __nv_bfloat16* __restrict__ queries, int n_q, int64_t ldq, float* __restrict__ out,
@@ -52,7 +54,7 @@ dense_scores_simt_kernel(const __nv_bfloat16* __restrict__ corpus, int64_t n_row
 #pragma unroll
             for (int j = 0; j < 4; ++j)
 #pragma unroll
-                for (int i = 0; i < 4; ++i) acc[j][i] = fmaf(a[i], b[j], acc[j][i]);
+                for (int i = 0; i < 4; ++i) acc[j][i] = SEP ? __fadd_rn(acc[j][i], __fmul_rn(b[j], a[i])) : fmaf(a[i], b[j], acc[j][i]);
         }
         __syncthreads();
     }
@@ -82,6 +84,7 @@ static size_t simt_workspace(int64_t n_rows, int n_queries, int k) {
     return align_up((size_t)qb * n_rows * 4, 256) + ezr_select_rows_workspace(qb, n_rows, k, EZR_F32);
 }
 
+template <bool SEP>
 static int simt_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
                      int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
                      float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
@@ -100,7 +103,7 @@ static int simt_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64
         dim3 grid(ceil_div(n_rows, kSimtTile), ceil_div(nq, kSimtTile));
         {
             ProfScope prof(EZR_PROF_DENSE_SIMT, st);
-            dense_scores_simt_kernel<<<grid, 256, 0, st>>>(corpus, n_rows, dim, ldc, queries + (int64_t)q0 * ldq, nq,
+            dense_scores_simt_kernel<SEP><<<grid, 256, 0, st>>>(corpus, n_rows, dim, ldc, queries + (int64_t)q0 * ldq, nq,
                                                            ldq, rows, n_rows);
         }
         EZR_LAUNCH_CHECK();
@@ -110,6 +113,26 @@ static int simt_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64
         if (rc) return rc;
     }
     return EZR_OK;
+}
+
+// Covers every call with at most n_queries queries, including a last query block smaller than the others (the
+// select workspace of fewer rows can be larger: it splits each row into more parts).
+size_t dense_exact_workspace(int64_t n_rows, int n_queries, int k) {
+    const int qb = simt_block_queries(n_rows, n_queries);
+    size_t sel = 0;
+    for (int m = 1; m <= qb; ++m) {
+        const size_t s = ezr_select_rows_workspace(m, n_rows, k, EZR_F32);
+        if (s > sel) sel = s;
+    }
+    return align_up((size_t)qb * n_rows * 4, 256) + sel;
+}
+
+int dense_exact_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
+                     int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
+                     float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
+                     cudaStream_t st) {
+    return simt_topk<true>(corpus, n_rows, dim, ldc, queries, n_queries, ldq, k, doc_group, q_group, id_base,
+                           out_scores, out_ids, out_counts, ws, ws_bytes, st);
 }
 
 static thread_local int g_force_kernel = 0;
@@ -208,7 +231,7 @@ int ezr_dense_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t
                              out_scores, out_ids, out_counts, workspace, workspace_bytes, st, form);
     }
     g_last_kernel = "simt";
-    return simt_topk(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k, doc_group, q_group, id_base, out_scores,
+    return simt_topk<false>(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k, doc_group, q_group, id_base, out_scores,
                      out_ids, out_counts, workspace, workspace_bytes, st);
 }
 

@@ -536,7 +536,7 @@ int encode_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t cols, uint6
     return EZR_OK;
 }
 
-static int tc_rows_per_slice(int64_t n_rows, int slices, int tn) {
+int tc_rows_per_slice(int64_t n_rows, int slices, int tn) {
     const int64_t tiles = (n_rows + tn - 1) / tn;
     return (int)((tiles + slices - 1) / slices) * tn;
 }
@@ -544,7 +544,7 @@ static int tc_rows_per_slice(int64_t n_rows, int slices, int tn) {
 // Number of corpus splits.  Units = splits x query blocks are walked by `sms` persistent CTAs.
 // Cost model: makespan = waves x (unit length + re-warm time of the per-thread top-k lists), in units of the time
 // one CTA needs to stream the whole corpus (~45 GB/s per SM); re-warming costs ~20 us per unit.
-static int ts_choose_splits(int qblocks, int64_t n_rows, int dim, int sms, int tn) {
+int ts_choose_splits(int qblocks, int64_t n_rows, int dim, int sms, int tn) {
     const int64_t tiles = (n_rows + tn - 1) / tn;
     int64_t max_s = tiles / 4;                 // at least 4 tiles per unit
     if (max_s > sms) max_s = sms;

@@ -17,6 +17,17 @@ int dense_tc_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t 
                                                 // 2: 64-query blocks and 128-row corpus tiles, 3: 2 in cluster pairs
 const char* dense_tc_form_name(int form);
 int dense_tc_max_qw(int dim);   // 2 while the 128-query block fits shared memory beside the ring (dim <= 768), else 1
+// corpus splits of the persistent work units (cost model in dense_tc.cu) and the rows of one split
+int ts_choose_splits(int qblocks, int64_t n_rows, int dim, int sms, int tn);
+int tc_rows_per_slice(int64_t n_rows, int slices, int tn);
+
+// Full scan with the rescore arithmetic of dense_s8.cu (fp32, increasing coordinate order, no FMA contraction):
+// score rows + ezr_select_rows (dense.cu).
+size_t dense_exact_workspace(int64_t n_rows, int n_queries, int k);
+int dense_exact_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
+                     int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
+                     float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
+                     cudaStream_t st);
 
 extern int g_dense_probe;       // see ezr_dense_set_probe
 extern int g_dense_stage_cap;   // see ezr_dense_set_stage_cap

@@ -347,21 +347,39 @@ def normalize_rows(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def check_quantizable(dim: int) -> None:
+    """The int8 scan (csrc/dense_s8.cu) takes 128-byte k-chunks of at most 1024 values."""
+    if dim % 128 != 0 or not 128 <= dim <= 1024:
+        raise ValueError(f"a quantized dense index needs dim % 128 == 0 and dim <= 1024 (got {dim})")
+
+
 class DenseIndex:
     """Row-major bf16 matrix of L2-normalised chunk embeddings (rows ``[row_lo, row_hi)`` of the corpus).
 
     The matrix lives in a buffer with spare capacity: :meth:`reserve` + :meth:`rows_for_append` hand out slices
     the encoder writes into directly (``embed_packed`` -> slice, no Python lists, no rebuild), :meth:`append`
     copies / normalises a block of new rows behind the existing ones in amortised O(new rows).
+
+    ``quantized=True`` keeps an int8 mirror of the rows (per-row scale, error and norm bounds, and the corpus-wide
+    maxima of the last two) in step with the bf16 rows: :func:`easyrag_b200.batched.dense_topk` then runs the
+    certified int8 pass + exact rescoring of ``ezr_dense_s8_topk``, which returns the same kind of exact result.
+    Rows written in place through :meth:`rows_for_append` are quantized at :meth:`commit`.  The quantized search is
+    currently slower than the bf16 one on unit-vector corpora (its certified margin admits too many candidates; see
+    the README) and synchronises its stream once per call.
     """
 
     def __init__(self, vectors: Optional[torch.Tensor], device=None, row_lo: int = 0,
                  doc_group: Optional[torch.Tensor] = None, normalize: bool = False, dim: Optional[int] = None,
-                 capacity: int = 0):
+                 capacity: int = 0, quantized: bool = False):
         _lib.require_cuda()
         device = torch.device(device if device is not None else "cuda")
         self.device = device
         self.row_lo = row_lo
+        self.quantized = bool(quantized)
+        if vectors is None and dim is None:
+            raise ValueError("DenseIndex: pass vectors or dim")
+        if self.quantized:
+            check_quantizable(dim if vectors is None else vectors.shape[1])
         if vectors is None:
             if dim is None:
                 raise ValueError("DenseIndex: pass vectors or dim")
@@ -381,11 +399,56 @@ class DenseIndex:
             self._buf = buf
             self.n_rows, self.dim = v.shape
         self.doc_group = None if doc_group is None else doc_group.to(device=device, dtype=torch.int32).contiguous()
+        if self.quantized:
+            self._alloc_mirror(self._buf.shape[0])
+            self._quantize(0, self.n_rows)
 
     @property
     def vectors(self) -> torch.Tensor:
         """The live rows (a view of the capacity buffer)."""
         return self._buf[:self.n_rows]
+
+    # ---- int8 mirror: rows, per-row scale / error bound / norm bound, maxima = [max error, max norm]
+    def _alloc_mirror(self, cap: int) -> None:
+        dev = self.device
+        self._s8 = torch.empty(cap, self.dim, dtype=torch.int8, device=dev)
+        self._scale = torch.empty(cap, dtype=torch.float32, device=dev)
+        self._err = torch.empty(cap, dtype=torch.float32, device=dev)
+        self._norm = torch.empty(cap, dtype=torch.float32, device=dev)
+        self.maxima = torch.zeros(2, dtype=torch.float32, device=dev)
+
+    def _quantize(self, lo: int, hi: int) -> None:
+        if hi <= lo:
+            return
+        x = self._buf[lo:hi]
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().ezr_dense_quantize_rows(
+                _lib.ptr(x), x.stride(0), hi - lo, self.dim, _lib.ptr(self._s8[lo:hi]), self._s8.stride(0),
+                _lib.ptr(self._scale[lo:hi]), _lib.ptr(self._err[lo:hi]), _lib.ptr(self._norm[lo:hi]),
+                _lib.ptr(self.maxima), _lib.stream_ptr()), "ezr_dense_quantize_rows")
+
+    @property
+    def rows_s8(self) -> torch.Tensor:
+        return self._s8[:self.n_rows]
+
+    @property
+    def row_scale(self) -> torch.Tensor:
+        return self._scale[:self.n_rows]
+
+    @property
+    def row_err(self) -> torch.Tensor:
+        return self._err[:self.n_rows]
+
+    @property
+    def row_norm(self) -> torch.Tensor:
+        return self._norm[:self.n_rows]
+
+    def index_bytes(self) -> int:
+        """Device bytes of the live rows (bf16, plus the int8 mirror and its per-row floats when quantized)."""
+        n = self.n_rows * self.dim * 2
+        if self.quantized:
+            n += self.n_rows * (self.dim + 12) + 8
+        return n
 
     def reserve(self, n_rows: int) -> None:
         """Make room for ``n_rows`` rows in total (geometric growth, one copy of the live rows when it grows)."""
@@ -395,6 +458,12 @@ class DenseIndex:
         buf = torch.empty(cap, self.dim, dtype=torch.bfloat16, device=self.device)
         buf[:self.n_rows].copy_(self._buf[:self.n_rows])
         self._buf = buf
+        if self.quantized:
+            old = (self._s8, self._scale, self._err, self._norm, self.maxima)
+            self._alloc_mirror(cap)
+            for dst, src in zip((self._s8, self._scale, self._err, self._norm), old[:4]):
+                dst[:self.n_rows].copy_(src[:self.n_rows])
+            self.maxima = old[4]
 
     def rows_for_append(self, n: int) -> torch.Tensor:
         """A writable [n, dim] bf16 slice right behind the live rows; call :meth:`commit` once it is filled."""
@@ -402,6 +471,8 @@ class DenseIndex:
         return self._buf[self.n_rows:self.n_rows + n]
 
     def commit(self, n: int) -> None:
+        if self.quantized:
+            self._quantize(self.n_rows, self.n_rows + n)
         self.n_rows += n
         self.doc_group = None            # per-row classes are rebuilt by the owner (they depend on the filter keys)
 
@@ -420,12 +491,26 @@ class DenseIndex:
         arrays = dict(vectors=self.vectors)
         if self.doc_group is not None:
             arrays["doc_group"] = self.doc_group
-        _save_arrays(path, dict(kind="dense", n_rows=self.n_rows, dim=self.dim, row_lo=self.row_lo), arrays)
+        if self.quantized:
+            arrays.update(rows_s8=self.rows_s8, row_scale=self.row_scale, row_err=self.row_err,
+                          row_norm=self.row_norm, maxima=self.maxima)
+        _save_arrays(path, dict(kind="dense", n_rows=self.n_rows, dim=self.dim, row_lo=self.row_lo,
+                                quantized=self.quantized), arrays)
 
     @classmethod
     def load(cls, path: str, device=None) -> "DenseIndex":
+        """A directory saved with the int8 mirror loads quantized (the mirror as saved); one without loads bf16."""
         meta, get = _load_arrays(path)
         if meta["kind"] != "dense":
             raise ValueError(f"{path}: not a dense index")
         dg = get("doc_group") if os.path.exists(os.path.join(path, "doc_group.npy")) else None
-        return cls(get("vectors"), device=device, row_lo=meta["row_lo"], doc_group=dg)
+        self = cls(get("vectors"), device=device, row_lo=meta["row_lo"], doc_group=dg)
+        if meta.get("quantized", False):
+            check_quantizable(self.dim)
+            self.quantized = True
+            self._alloc_mirror(self._buf.shape[0])
+            for dst, name in ((self._s8, "rows_s8"), (self._scale, "row_scale"), (self._err, "row_err"),
+                              (self._norm, "row_norm")):
+                dst[:self.n_rows].copy_(get(name))
+            self.maxima.copy_(get("maxima"))
+        return self

@@ -126,8 +126,10 @@ class B200VectorStore:
     Python float lists between the encoder and the index.
     """
 
-    def __init__(self, nodes: Optional[Sequence[Any]] = None, device="cuda"):
+    def __init__(self, nodes: Optional[Sequence[Any]] = None, device="cuda", quantize: bool = False):
         self.device = device
+        # keep an int8 mirror: exact search through a certified int8 pass (currently slower than bf16, README)
+        self.quantize = bool(quantize)
         self.nodes: List[Any] = []
         self.index: Optional[DenseIndex] = None
         self._groups: Optional[_GroupTable] = None
@@ -138,7 +140,7 @@ class B200VectorStore:
 
     def _ensure_index(self, dim: int) -> DenseIndex:
         if self.index is None:
-            self.index = DenseIndex(None, device=self.device, dim=dim)
+            self.index = DenseIndex(None, device=self.device, dim=dim, quantized=self.quantize)
             self._ws = batched.Workspace(self.index.device)
         elif self.index.dim != dim:
             raise ValueError(f"embedding dim {dim} != collection dim {self.index.dim}")
@@ -168,11 +170,11 @@ class B200VectorStore:
         return self._registered(nodes)
 
     @classmethod
-    def from_embed_model(cls, nodes: Sequence[Any], embed_model, device="cuda", batch_size: Optional[int] = None
-                         ) -> "B200VectorStore":
+    def from_embed_model(cls, nodes: Sequence[Any], embed_model, device="cuda", batch_size: Optional[int] = None,
+                         quantize: bool = False) -> "B200VectorStore":
         """Corpus encode written in place (replaces pipeline.py:141-158 + ingestion.py:155-191): every batch of
         ``embed_model.embed_tensor`` lands in its slice of the corpus matrix, normalised on the way."""
-        store = cls(device=device)
+        store = cls(device=device, quantize=quantize)
         nodes = list(nodes)
         bs = int(batch_size or getattr(embed_model, "embed_batch_size", 128) or 128)
         embed_type = getattr(embed_model, "_embed_type", 0)

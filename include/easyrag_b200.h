@@ -13,8 +13,9 @@
  *     ezr_last_error() returns a thread-local message for the last failure.
  *   - all pointers are DEVICE pointers unless the name ends in _host.
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
- *   - launch functions never synchronise and never allocate: outputs and the
- *     workspace are caller-owned (query the size with the *_workspace call).
+ *   - launch functions never allocate: outputs and the workspace are caller-owned
+ *     (query the size with the *_workspace call).  They do not synchronise, except
+ *     where a function says so (ezr_dense_s8_topk, the rerank packers below).
  *   - document ids are int32, local to the shard the index was built over;
  *     `id_base` is added on output so a row-sharded corpus yields global ids.
  *   - canonical rank order everywhere: score descending, then id descending
@@ -225,6 +226,35 @@ int ezr_dense_set_stage_cap(int32_t stages);
  * insertion path. */
 int ezr_dense_set_probe(int32_t probe);
 
+/* Dense top-k over an int8 copy of the corpus (easyrag_b200/csrc/dense_s8.cu has the definition and the bound).
+ * The result is the canonical top-k under rescore(q, r): the fp32 dot product of the bf16 query and bf16 row in
+ * increasing coordinate order, one __fmul_rn and one __fadd_rn per coordinate (no FMA contraction), -0.0 returned
+ * as +0.0, over every row that passes the filter -- never an approximation.
+ *
+ * quantize_rows: per row of bf16 x, scale = max|x_i| / 127 (fp32), out_s8 = clamp(rint(x_i / scale), +-127) (a zero
+ * row: scale 0, R 0), err and norm = ||x - scale R||_2 and ||scale R||_2 evaluated in fp64 and rounded up to fp32 (the
+ * bound of dense_s8.cu allows for the fp64 rounding).  Strides in
+ * elements, as ezr_normalize_rows.  maxima (device float[2] = {max err, max norm}, may be NULL) is raised atomically:
+ * zero it before the first rows of an index, keep it across appends. */
+int ezr_dense_quantize_rows(const void* x_bf16, int64_t ldx, int64_t n_rows, int32_t dim, int8_t* out_s8, int64_t ldo,
+                            float* scale, float* err, float* norm, float* maxima, void* stream);
+/* The arguments of ezr_dense_topk, plus the int8 rows (ld_s8 in bytes, a multiple of 16), their per-row scales, the
+ * maxima of quantize_rows, and out_cand_counts ([n_queries] or NULL: candidates the int8 pass emitted per query;
+ * more than the capacity = overflowed, answered by the full scan; an overflowed query stops emitting, so its count
+ * then only tells that it overflowed).  dim % 128 == 0, dim <= 1024; k <= 16 runs the
+ * int8 pass + rescoring, 16 < k <= 1024 the full scan.  The call waits for the int8 pass to learn how many queries
+ * overflowed (one stream synchronisation). */
+size_t ezr_dense_s8_topk_workspace(int64_t n_rows, int32_t dim, int32_t n_queries, int32_t k);
+int ezr_dense_s8_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t ld_corpus,
+                      const void* queries_bf16, int32_t n_queries, int64_t ld_queries, int32_t k,
+                      const int32_t* doc_group, const int32_t* q_group, int32_t id_base, float* out_scores,
+                      int32_t* out_ids, int32_t* out_counts, const int8_t* corpus_s8, int64_t ld_s8,
+                      const float* row_scale, const float* maxima, int32_t* out_cand_counts, void* workspace,
+                      size_t workspace_bytes, void* stream);
+/* Candidates per query the int8 pass may buffer (0 = the default, 4096).  Results never depend on it: a query that
+ * emits more is answered by the full scan.  The workspace size depends on it; query the workspace after setting. */
+int ezr_dense_s8_set_capacity(int32_t cap);   /* per host thread */
+
 /* ------------------------------------------------------------- fusion ---
  * HybridRetriever.reciprocal_rank_fusion (retrievers.py:256-274): list a first, then list b
  * (the reference passes [sparse, dense], retrievers.py:290); score += 1/(rank+K), rank from 1, fp64;
@@ -376,7 +406,10 @@ typedef enum ezr_prof_slot {
     EZR_PROF_ENC_OTHER = 7,  /* encoder norms / elementwise */
     EZR_PROF_BM25_CAND = 8,  /* bm25_cand_kernel (integer candidate pass over packed postings) */
     EZR_PROF_BM25_RESCORE = 9, /* bm25_rescore_kernel (exact float64 rescoring + top-k of the candidates) */
-    EZR_PROF_COUNT = 10
+    EZR_PROF_DENSE_S8_SCAN = 10,    /* dense_s8_prep_kernel + dense_s8_scan_kernel (int8 candidate pass) */
+    EZR_PROF_DENSE_S8_RESCORE = 11, /* dense_s8_rescore_kernel (exact rescoring + top-k of the candidates) */
+    EZR_PROF_DENSE_S8_FULL = 12,    /* full scan of overflowed queries / k > 16 (gather + score rows + select) */
+    EZR_PROF_COUNT = 13
 } ezr_prof_slot;
 /* kernels launched by this library since it was loaded (every launch site counts itself) */
 long long ezr_launch_count(void);
