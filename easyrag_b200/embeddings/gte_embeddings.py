@@ -3,7 +3,8 @@
 Same constructor (``model_name``, ``embed_type``, ``embed_batch_size`` ...), same methods; the Qwen2 forward,
 last-token pooling and L2 normalisation run in the CUDA kernels of easyrag_b200/encoder.py instead of
 torch/cuBLAS.  Two keyword-only extras exist because this build is offline: ``encoder=`` (a ready
-``Qwen2Encoder``) and ``tokenizer=`` (anything callable like a HF tokenizer).
+``Qwen2Encoder``) and ``tokenizer=`` (anything callable like a HF tokenizer).  ``precision="fp8"`` builds the encoder
+with e4m3 layer GEMMs (Qwen2Encoder); the default "bf16" is the unchanged path.
 """
 from __future__ import annotations
 
@@ -11,7 +12,7 @@ from typing import Any, List
 
 import torch
 
-from ..encoder import PackedBatch, Qwen2Config, Qwen2Encoder
+from ..encoder import PackedBatch, Qwen2Config, Qwen2Encoder, _check_precision
 from ..retrievers import get_node_content
 from ..schema import BaseEmbedding, PrivateAttr
 from . import _loading
@@ -23,9 +24,14 @@ class GTEEmbedding(BaseEmbedding):
     _tokenizer: Any = PrivateAttr()
     _device: str = PrivateAttr()
     _embed_type: int = PrivateAttr()
+    _precision: str = PrivateAttr()
 
     def __init__(self, model_name: str = None, embed_type: int = 0, encoder: Qwen2Encoder = None, tokenizer=None,
-                 device: str = "cuda", **kwargs: Any) -> None:
+                 device: str = "cuda", precision: str = "bf16", **kwargs: Any) -> None:
+        _check_precision(precision)
+        given = getattr(encoder, "precision", "bf16")
+        if encoder is not None and given != precision:
+            raise ValueError(f"precision={precision!r} but the given encoder runs {given!r}")
         if encoder is None:
             cfgd = _loading.load_config(model_name)
             cfg = Qwen2Config(vocab_size=cfgd["vocab_size"], hidden_size=cfgd["hidden_size"],
@@ -34,7 +40,8 @@ class GTEEmbedding(BaseEmbedding):
                               num_key_value_heads=cfgd.get("num_key_value_heads", cfgd["num_attention_heads"]),
                               max_position_embeddings=min(cfgd.get("max_position_embeddings", 8192), 32768),
                               rms_norm_eps=cfgd.get("rms_norm_eps", 1e-6), rope_theta=cfgd.get("rope_theta", 10000.0))
-            encoder = Qwen2Encoder(cfg, _loading.strip_prefix(_loading.load_state_dict(model_name)), device=device)
+            encoder = Qwen2Encoder(cfg, _loading.strip_prefix(_loading.load_state_dict(model_name)), device=device,
+                                   precision=precision)
         if tokenizer is None:
             tokenizer = _loading.load_tokenizer(model_name)
         kwargs.setdefault("model_name", model_name or "gte-qwen2")
@@ -43,6 +50,7 @@ class GTEEmbedding(BaseEmbedding):
         self._tokenizer = tokenizer
         self._device = str(encoder.device)
         self._embed_type = embed_type
+        self._precision = precision
 
     def get_detailed_instruct(self, query: str) -> str:
         """gte_embeddings.py:52-53."""

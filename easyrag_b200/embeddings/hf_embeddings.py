@@ -2,7 +2,8 @@
 
 The reference wraps ``SentenceTransformer(model_name).encode(..., normalize_embeddings=True)``; here the BERT-shaped
 encoder, pooling and normalisation run in easyrag_b200/encoder.py's CUDA kernels.  Same constructor arguments
-(including the rejection of the deprecated ones, hf_embeddings.py:67-78) and methods.
+(including the rejection of the deprecated ones, hf_embeddings.py:67-78) and methods.  ``precision="fp8"`` builds
+the encoder with e4m3 layer GEMMs (BertEncoder); the default "bf16" is the unchanged path.
 """
 from __future__ import annotations
 
@@ -12,7 +13,7 @@ from typing import Any, List, Optional
 
 import torch
 
-from ..encoder import BertConfig, BertEncoder, PackedBatch
+from ..encoder import BertConfig, BertEncoder, PackedBatch, _check_precision
 from ..retrievers import get_node_content
 from ..schema import BaseEmbedding, Field, PrivateAttr
 from . import _loading
@@ -62,6 +63,7 @@ class HuggingFaceEmbedding(BaseEmbedding):
     _prompts: Any = PrivateAttr()
     _device: str = PrivateAttr()
     _embed_type: int = PrivateAttr()
+    _precision: str = PrivateAttr()
 
     def __init__(self, model_name: str = DEFAULT_HUGGINGFACE_EMBEDDING_MODEL, tokenizer_name: Optional[str] = "deprecated",
                  pooling: str = "deprecated", max_length: Optional[int] = None, query_instruction: Optional[str] = None,
@@ -69,8 +71,12 @@ class HuggingFaceEmbedding(BaseEmbedding):
                  tokenizer: Optional[Any] = "deprecated", embed_batch_size: int = DEFAULT_EMBED_BATCH_SIZE,
                  cache_folder: Optional[str] = None, trust_remote_code: bool = False, device: Optional[str] = None,
                  callback_manager=None, embed_type: int = 0, encoder: BertEncoder = None, hf_tokenizer=None,
-                 **model_kwargs):
+                 precision: str = "bf16", **model_kwargs):
         device = device or "cuda"
+        _check_precision(precision)
+        given = getattr(encoder, "precision", "bf16")
+        if encoder is not None and given != precision:
+            raise ValueError(f"precision={precision!r} but the given encoder runs {given!r}")
         for variable, value in [("model", model), ("tokenizer", tokenizer), ("pooling", pooling),
                                 ("tokenizer_name", tokenizer_name)]:
             if value != "deprecated":
@@ -85,7 +91,7 @@ class HuggingFaceEmbedding(BaseEmbedding):
                              max_position_embeddings=c.get("max_position_embeddings", 512),
                              layer_norm_eps=c.get("layer_norm_eps", 1e-12))
             encoder = BertEncoder(cfg, _loading.strip_prefix(_loading.load_state_dict(model_name)),
-                                  device=device, pooling=_pooling_from_dir(model_name))
+                                  device=device, pooling=_pooling_from_dir(model_name), precision=precision)
         max_pos = int(encoder.cfg.max_position_embeddings)
         max_length = max_length or min(DEFAULT_HUGGINGFACE_LENGTH, max_pos)
         if max_length > max_pos:
@@ -97,6 +103,7 @@ class HuggingFaceEmbedding(BaseEmbedding):
                          text_instruction=text_instruction, cache_folder=cache_folder)
         self._device = device
         self._embed_type = embed_type
+        self._precision = precision
         self._model = encoder
         self._tok = hf_tokenizer if hf_tokenizer is not None else _loading.load_tokenizer(model_name)
         self._prompts = {"query": query_instruction or get_query_instruct_for_model_name(model_name),

@@ -75,6 +75,82 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
     return out
 
 
+def gemm_fp8(a8: torch.Tensor, sa: torch.Tensor, w8: torch.Tensor, sw: torch.Tensor, bias: Optional[torch.Tensor] = None,
+             residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+             epilogue: int = EPI_NONE) -> torch.Tensor:
+    """out = epi(diag(sa) a8 @ w8.T diag(sw) + bias) (+ residual);  a8 [M,K], w8 [N,K] float8_e4m3fn, sa [M] / sw [N]
+    float32 power-of-two scales (quant_rows / quant_weight).  SwiGLU weights interleave gate / up rows per 64
+    (``_interleave_gate_up(.., block=64)``)."""
+    L = _lib.lib()
+    m, k = a8.shape
+    n = w8.shape[0]
+    n_out = n // 2 if epilogue == EPI_SWIGLU else n
+    if out is None:
+        out = torch.empty(m, n_out, dtype=torch.bfloat16, device=a8.device)
+    _lib.check(L.ezr_gemm_fp8(_lib.ptr(a8), _lib.ptr(sa), m, k, a8.stride(0), _lib.ptr(w8), _lib.ptr(sw), n, w8.stride(0),
+                              _lib.ptr(bias), _lib.ptr(residual), residual.stride(0) if residual is not None else 0,
+                              _lib.ptr(out), out.stride(0), epilogue, _lib.stream_ptr()), "ezr_gemm_fp8")
+    return out
+
+
+def _fp8_dest(x: torch.Tensor, out8: Optional[torch.Tensor], scale: Optional[torch.Tensor]):
+    if out8 is None:
+        out8 = torch.empty(x.shape, dtype=torch.float8_e4m3fn, device=x.device)
+    if scale is None:
+        scale = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
+    return out8, scale
+
+
+def quant_rows(x: torch.Tensor, out8: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None
+               ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """bf16 [rows, cols] -> (e4m3 [rows, cols], float32 [rows]): one power-of-two scale per row (ezr_quant_rows_fp8)."""
+    L = _lib.lib()
+    out8, scale = _fp8_dest(x, out8, scale)
+    _lib.check(L.ezr_quant_rows_fp8(_lib.ptr(x), x.stride(0), x.shape[0], x.shape[1], _lib.ptr(out8), out8.stride(0),
+                                    _lib.ptr(scale), _lib.stream_ptr()), "ezr_quant_rows_fp8")
+    return out8, scale
+
+
+def quant_weight(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """nn.Linear weight bf16 [n, k] -> (e4m3 [n, k], float32 [n]): one power-of-two scale per output channel."""
+    L = _lib.lib()
+    w8, scale = _fp8_dest(w, None, None)
+    _lib.check(L.ezr_quant_weight_fp8(_lib.ptr(w), w.stride(0), w.shape[0], w.shape[1], _lib.ptr(w8), w8.stride(0),
+                                      _lib.ptr(scale), _lib.stream_ptr()), "ezr_quant_weight_fp8")
+    return w8, scale
+
+
+def rmsnorm_fp8(x: torch.Tensor, gamma: torch.Tensor, eps: float, out8: Optional[torch.Tensor] = None,
+                scale: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None):
+    """rmsnorm's bf16 row (also stored to ``out`` when given), quantised per row -> (e4m3, float32 scales)."""
+    L = _lib.lib()
+    out8, scale = _fp8_dest(x, out8, scale)
+    _lib.check(L.ezr_rmsnorm_fp8(_lib.ptr(x), x.stride(0), _lib.ptr(gamma), eps, x.shape[0], x.shape[1], _lib.ptr(out),
+                                 out.stride(0) if out is not None else 0, _lib.ptr(out8), out8.stride(0), _lib.ptr(scale),
+                                 _lib.stream_ptr()), "ezr_rmsnorm_fp8")
+    return out8, scale
+
+
+def layernorm_fp8(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float,
+                  out8: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None,
+                  out: Optional[torch.Tensor] = None):
+    """layernorm's bf16 row (also stored to ``out`` when given), quantised per row -> (e4m3, float32 scales)."""
+    L = _lib.lib()
+    out8, scale = _fp8_dest(x, out8, scale)
+    _lib.check(L.ezr_layernorm_fp8(_lib.ptr(x), x.stride(0), _lib.ptr(gamma), _lib.ptr(beta), eps, x.shape[0],
+                                   x.shape[1], _lib.ptr(out), out.stride(0) if out is not None else 0, _lib.ptr(out8),
+                                   out8.stride(0), _lib.ptr(scale), _lib.stream_ptr()), "ezr_layernorm_fp8")
+    return out8, scale
+
+
+PRECISIONS = ("bf16", "fp8")
+
+
+def _check_precision(precision: str) -> None:
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
+
+
 def _dest(out_bf16: Optional[torch.Tensor], n: int, d: int, device) -> torch.Tensor:
     if out_bf16 is None:
         return torch.empty(n, d, dtype=torch.bfloat16, device=device)
@@ -159,23 +235,36 @@ def _bf16(t: torch.Tensor, device) -> torch.Tensor:
     return t.detach().to(device=device, dtype=torch.bfloat16).contiguous()
 
 
-def _interleave_gate_up(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
-    """[ffn, d] x2 -> [2*ffn, d] in blocks of 128 gate rows followed by the matching 128 up rows (SwiGLU epilogue:
-    one 256-column GEMM tile holds both halves of the same 128 outputs)."""
+def _weight(t: torch.Tensor, device, precision: str):
+    """A layer weight as the GEMMs of ``precision`` take it: bf16, or (e4m3, per-channel scales) with no bf16 copy kept."""
+    w = _bf16(t, device)
+    return w if precision == "bf16" else quant_weight(w)
+
+
+def _interleave_gate_up(gate: torch.Tensor, up: torch.Tensor, block: int = 128) -> torch.Tensor:
+    """[ffn, d] x2 -> [2*ffn, d] in blocks of ``block`` gate rows followed by the matching ``block`` up rows (SwiGLU
+    epilogue: one GEMM tile holds both halves of the same outputs; 128 for the bf16 kernel's 256-column tiles, 64 for
+    the fp8 kernel's 128-column tiles)."""
     ffn, d = gate.shape
     if ffn % 128:
         raise ValueError("intermediate_size must be a multiple of 128")
-    g = gate.view(ffn // 128, 128, d)
-    u = up.view(ffn // 128, 128, d)
+    g = gate.view(ffn // block, block, d)
+    u = up.view(ffn // block, block, d)
     return torch.stack([g, u], dim=1).reshape(2 * ffn, d).contiguous()
 
 
 class Qwen2Encoder:
-    """Bidirectional Qwen2 stack + last-token pooling + L2 norm == GTEEmbedding._embed's model part."""
+    """Bidirectional Qwen2 stack + last-token pooling + L2 norm == GTEEmbedding._embed's model part.
 
-    def __init__(self, cfg: Qwen2Config, state: Dict[str, torch.Tensor], device="cuda"):
+    ``precision="fp8"`` holds the layer weights as e4m3 with per-channel scales only and runs every layer GEMM on
+    the e4m3 kernel (activations quantised per row); embeddings, norms, attention, RoPE, pooling and the residual
+    stream stay bf16.  Lossy: see DESIGN.md 4.5a for its error bound."""
+
+    def __init__(self, cfg: Qwen2Config, state: Dict[str, torch.Tensor], device="cuda", precision: str = "bf16"):
+        _check_precision(precision)
         _lib.require_cuda()
         self.cfg = cfg
+        self.precision = precision
         self.device = torch.device(device)
         if cfg.head_dim not in (64, 128):
             raise ValueError("head_dim must be 64 or 128")
@@ -189,11 +278,13 @@ class Qwen2Encoder:
                               g(p + "self_attn.v_proj.weight")], 0)
             bqkv = torch.cat([g(p + "self_attn.q_proj.bias"), g(p + "self_attn.k_proj.bias"),
                               g(p + "self_attn.v_proj.bias")], 0)
+            block = 128 if precision == "bf16" else 64
+            wgu = _interleave_gate_up(g(p + "mlp.gate_proj.weight").float(), g(p + "mlp.up_proj.weight").float(), block)
             self.layers.append(dict(
-                ln1=_bf16(g(p + "input_layernorm.weight"), dev), wqkv=_bf16(wqkv, dev), bqkv=_bf16(bqkv, dev),
-                wo=_bf16(g(p + "self_attn.o_proj.weight"), dev), ln2=_bf16(g(p + "post_attention_layernorm.weight"), dev),
-                wgu=_bf16(_interleave_gate_up(g(p + "mlp.gate_proj.weight").float(), g(p + "mlp.up_proj.weight").float()), dev),
-                wdown=_bf16(g(p + "mlp.down_proj.weight"), dev)))
+                ln1=_bf16(g(p + "input_layernorm.weight"), dev), wqkv=_weight(wqkv, dev, precision),
+                bqkv=_bf16(bqkv, dev), wo=_weight(g(p + "self_attn.o_proj.weight"), dev, precision),
+                ln2=_bf16(g(p + "post_attention_layernorm.weight"), dev), wgu=_weight(wgu, dev, precision),
+                wdown=_weight(g(p + "mlp.down_proj.weight"), dev, precision)))
         self.norm = _bf16(g("norm.weight"), dev)
         # rotary tables exactly as Qwen2RotaryEmbedding builds them (modeling_qwen.py:100-133): fp32 math, cast to bf16
         hd = cfg.head_dim
@@ -221,6 +312,9 @@ class Qwen2Encoder:
             qkv = torch.empty(t, (H + 2 * KV) * hd, dtype=torch.bfloat16, device=dev)
             ao = torch.empty(t, H * hd, dtype=torch.bfloat16, device=dev)
             act = torch.empty(t, cfg.intermediate_size, dtype=torch.bfloat16, device=dev)
+            if self.precision == "fp8":
+                self._layers_fp8(batch, x, qkv, ao, act)
+                return x
             for ly in self.layers:
                 rmsnorm(x, ly["ln1"], cfg.rms_norm_eps, out=xn)
                 gemm(xn, ly["wqkv"], bias=ly["bqkv"], out=qkv)
@@ -232,6 +326,30 @@ class Qwen2Encoder:
                 gemm(xn, ly["wgu"], out=act, epilogue=EPI_SWIGLU)
                 gemm(act, ly["wdown"], residual=x, out=x)
         return x
+
+    def _layers_fp8(self, batch: PackedBatch, x, qkv, ao, act) -> None:
+        """The layer loop of ``hidden`` on the e4m3 GEMMs: the norms quantise their bf16 output in the same kernel, the
+        attention output and the SwiGLU output are quantised per row before o_proj / down_proj."""
+        L = _lib.lib()
+        cfg = self.cfg
+        t = x.shape[0]
+        H, KV, hd = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+        st = _lib.stream_ptr()
+        x8, xs = _fp8_dest(x, None, None)
+        a8, as_ = _fp8_dest(ao, None, None)
+        act8, acts = _fp8_dest(act, None, None)
+        for ly in self.layers:
+            rmsnorm_fp8(x, ly["ln1"], cfg.rms_norm_eps, out8=x8, scale=xs)
+            gemm_fp8(x8, xs, *ly["wqkv"], bias=ly["bqkv"], out=qkv)
+            _lib.check(L.ezr_rope(_lib.ptr(qkv), qkv.stride(0), _lib.ptr(batch.positions), _lib.ptr(self.cos),
+                                  _lib.ptr(self.sin), cfg.max_position_embeddings, H + KV, hd, t, st), "ezr_rope")
+            attention(qkv, batch.cu, batch.max_len, H, KV, hd, out=ao)
+            quant_rows(ao, a8, as_)
+            gemm_fp8(a8, as_, *ly["wo"], residual=x, out=x)
+            rmsnorm_fp8(x, ly["ln2"], cfg.rms_norm_eps, out8=x8, scale=xs)
+            gemm_fp8(x8, xs, *ly["wgu"], out=act, epilogue=EPI_SWIGLU)
+            quant_rows(act, act8, acts)
+            gemm_fp8(act8, acts, *ly["wdown"], residual=x, out=x)
 
     @torch.no_grad()
     def embed_packed(self, batch: PackedBatch, out_bf16: Optional[torch.Tensor] = None
@@ -279,11 +397,16 @@ class BertEncoder:
     """BERT encoder + CLS/mean pooling + L2 norm == what SentenceTransformer.encode runs for bge-* / gte-base.
 
     ``state`` uses transformers.BertModel parameter names (``embeddings.*``, ``encoder.layer.N.*``).
+    ``precision="fp8"``: the layer GEMMs on e4m3 weights (per-channel scales, no bf16 copy kept) and per-row quantised
+    activations, as in Qwen2Encoder; everything else stays bf16.
     """
 
-    def __init__(self, cfg: BertConfig, state: Dict[str, torch.Tensor], device="cuda", pooling: str = "cls"):
+    def __init__(self, cfg: BertConfig, state: Dict[str, torch.Tensor], device="cuda", pooling: str = "cls",
+                 precision: str = "bf16"):
+        _check_precision(precision)
         _lib.require_cuda()
         self.cfg = cfg
+        self.precision = precision
         self.device = torch.device(device)
         if cfg.head_dim not in (64, 128):
             raise ValueError("head_dim must be 64 or 128")
@@ -304,12 +427,14 @@ class BertEncoder:
             bqkv = torch.cat([g(p + "attention.self.query.bias"), g(p + "attention.self.key.bias"),
                               g(p + "attention.self.value.bias")], 0)
             self.layers.append(dict(
-                wqkv=_bf16(wqkv, dev), bqkv=_bf16(bqkv, dev),
-                wo=_bf16(g(p + "attention.output.dense.weight"), dev), bo=_bf16(g(p + "attention.output.dense.bias"), dev),
+                wqkv=_weight(wqkv, dev, precision), bqkv=_bf16(bqkv, dev),
+                wo=_weight(g(p + "attention.output.dense.weight"), dev, precision),
+                bo=_bf16(g(p + "attention.output.dense.bias"), dev),
                 ln1g=_bf16(g(p + "attention.output.LayerNorm.weight"), dev),
                 ln1b=_bf16(g(p + "attention.output.LayerNorm.bias"), dev),
-                w1=_bf16(g(p + "intermediate.dense.weight"), dev), b1=_bf16(g(p + "intermediate.dense.bias"), dev),
-                w2=_bf16(g(p + "output.dense.weight"), dev), b2=_bf16(g(p + "output.dense.bias"), dev),
+                w1=_weight(g(p + "intermediate.dense.weight"), dev, precision),
+                b1=_bf16(g(p + "intermediate.dense.bias"), dev),
+                w2=_weight(g(p + "output.dense.weight"), dev, precision), b2=_bf16(g(p + "output.dense.bias"), dev),
                 ln2g=_bf16(g(p + "output.LayerNorm.weight"), dev), ln2b=_bf16(g(p + "output.LayerNorm.bias"), dev)))
 
     @torch.no_grad()
@@ -338,6 +463,9 @@ class BertEncoder:
             ao = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
             y = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
             act = torch.empty(t, cfg.intermediate_size, dtype=torch.bfloat16, device=dev)
+            if self.precision == "fp8":
+                self._layers_fp8(batch, x, qkv, ao, y, act)
+                return x
             for ly in self.layers:
                 gemm(x, ly["wqkv"], bias=ly["bqkv"], out=qkv)
                 attention(qkv, batch.cu, batch.max_len, H, H, hd, out=ao)
@@ -347,6 +475,25 @@ class BertEncoder:
                 gemm(act, ly["w2"], bias=ly["b2"], residual=x, out=y)
                 layernorm(y, ly["ln2g"], ly["ln2b"], cfg.layer_norm_eps, out=x)
         return x
+
+    def _layers_fp8(self, batch: PackedBatch, x, qkv, ao, y, act) -> None:
+        """The layer loop of ``hidden`` on the e4m3 GEMMs.  x (bf16, the residual stream) and its e4m3 copy x8 come
+        out of the same LayerNorm kernel; the attention and GELU outputs are quantised per row."""
+        cfg = self.cfg
+        H, hd = cfg.num_attention_heads, cfg.head_dim
+        x8, xs = quant_rows(x)
+        a8, as_ = _fp8_dest(ao, None, None)
+        act8, acts = _fp8_dest(act, None, None)
+        for ly in self.layers:
+            gemm_fp8(x8, xs, *ly["wqkv"], bias=ly["bqkv"], out=qkv)
+            attention(qkv, batch.cu, batch.max_len, H, H, hd, out=ao)
+            quant_rows(ao, a8, as_)
+            gemm_fp8(a8, as_, *ly["wo"], bias=ly["bo"], residual=x, out=y)
+            layernorm_fp8(y, ly["ln1g"], ly["ln1b"], cfg.layer_norm_eps, out8=x8, scale=xs, out=x)
+            gemm_fp8(x8, xs, *ly["w1"], bias=ly["b1"], out=act, epilogue=EPI_GELU)
+            quant_rows(act, act8, acts)
+            gemm_fp8(act8, acts, *ly["w2"], bias=ly["b2"], residual=x, out=y)
+            layernorm_fp8(y, ly["ln2g"], ly["ln2b"], cfg.layer_norm_eps, out8=x8, scale=xs, out=x)
 
     @torch.no_grad()
     def embed_packed(self, batch: PackedBatch, normalize: bool = True, out_bf16: Optional[torch.Tensor] = None

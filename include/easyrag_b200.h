@@ -353,6 +353,30 @@ int ezr_cross_order_topk(const float* sig, const int32_t* pair_off, int32_t n_qu
 int ezr_gemm_bf16(const void* a, int32_t m, int32_t k, int64_t lda, const void* w, int32_t n, int64_t ldw,
                   const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo, int32_t epilogue,
                   void* stream);
+/* FP8 (opt-in precision of the encoders).  e4m3 operands, fp32 accumulation promoted every 128 K, bf16 output:
+ *   out[M,N'] = epi(diag(sa) . A8[M,K] . W8[N,K]^T . diag(sw) + bias) (+ residual)
+ * sa float32 [M] (one power-of-two scale per activation row), sw float32 [N] (one per weight row / output channel),
+ * epilogues as ezr_gemm_bf16 except SwiGLU: W8 (and bias) rows interleaved per 128: 64 gate rows then the matching
+ * 64 up rows.  K % 128 == 0; lda, ldw (bytes) multiples of 16; A8 / W8 16-byte aligned.  out may alias residual. */
+int ezr_gemm_fp8(const void* a8, const float* sa, int32_t m, int32_t k, int64_t lda, const void* w8, const float* sw,
+                 int32_t n, int64_t ldw, const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo,
+                 int32_t epilogue, void* stream);
+/* bf16 [rows, cols] -> e4m3 [rows, cols] (row stride ldo bytes) and float32 scales [rows]: per row
+ * s = 2^ceil(log2(amax / 448)) (1 for an all-zero row), q = e4m3_rn(x / s).  One warp per row.  cols, ldx, ldo
+ * multiples of 8; x 16-byte, out 8-byte aligned.  Inf / NaN inputs are not supported. */
+int ezr_quant_rows_fp8(const void* x, int64_t ldx, int32_t rows, int32_t cols, void* out_e4m3, int64_t ldo,
+                       float* out_scale, void* stream);
+/* the same for an nn.Linear weight [n, k]: one scale per output channel (row); run once when a model loads */
+int ezr_quant_weight_fp8(const void* w, int64_t ldw, int32_t n, int32_t k, void* out_e4m3, int64_t ldo,
+                         float* out_scale, void* stream);
+/* ezr_rmsnorm / ezr_layernorm rounded to bf16 exactly as they are, stored to out when out != NULL, and that bf16 row
+ * quantised as ezr_quant_rows_fp8 does, in the same kernel.  dim % 8 == 0, dim <= 4096; x / out / gamma / beta
+ * 16-byte aligned, out_e4m3 8-byte aligned, strides multiples of 8. */
+int ezr_rmsnorm_fp8(const void* x, int64_t ldx, const void* gamma, float eps, int32_t n_rows, int32_t dim, void* out,
+                    int64_t ldo, void* out_e4m3, int64_t ldq, float* out_scale, void* stream);
+int ezr_layernorm_fp8(const void* x, int64_t ldx, const void* gamma, const void* beta, float eps, int32_t n_rows,
+                      int32_t dim, void* out, int64_t ldo, void* out_e4m3, int64_t ldq, float* out_scale,
+                      void* stream);
 /* non-causal attention over packed q|k|v rows ([n_tokens, (H + 2*KV) * hd], row stride ld); head_dim 64 or 128; GQA
  * via n_kv_heads.  Default kernel: wgmma (S = QK^T and O += PV on the tensor cores, S/P/O in registers,
  * Q/K/V tiles by TMA).  n_tokens bounds the TMA tensor map (tiles that run past the last token are zero-filled). */
