@@ -90,6 +90,7 @@ SIGNATURES = {
     "ezr_rmsnorm_fp8": (C.c_int, [_p, _i64, _p, C.c_float, _i32, _i32, _p, _i64, _p, _i64, _p, _p]),
     "ezr_layernorm_fp8": (C.c_int, [_p, _i64, _p, _p, C.c_float, _i32, _i32, _p, _i64, _p, _i64, _p, _p]),
     "ezr_attn_bidir": (C.c_int, [_p, _i64, _i64, _p, _i32, _i32, _i32, _i32, _i32, C.c_float, _p, _i64, _p]),
+    "ezr_attn_causal": (C.c_int, [_p, _i64, _i64, _p, _i32, _i32, _i32, _i32, _i32, C.c_float, _p, _i64, _p]),
     "ezr_attn_set_kernel": (C.c_int, [_i32]),
     "ezr_attn_last_kernel": (C.c_char_p, []),
     "ezr_embed_gather": (C.c_int, [_p, _i32, _p, _i64, _i32, _i32, _p, _i64, _p]),

@@ -4,7 +4,8 @@ Same constructor (``model_name``, ``embed_type``, ``embed_batch_size`` ...), sam
 last-token pooling and L2 normalisation run in the CUDA kernels of easyrag_b200/encoder.py instead of
 torch/cuBLAS.  Two keyword-only extras exist because this build is offline: ``encoder=`` (a ready
 ``Qwen2Encoder``) and ``tokenizer=`` (anything callable like a HF tokenizer).  ``precision="fp8"`` builds the encoder
-with e4m3 layer GEMMs (Qwen2Encoder); the default "bf16" is the unchanged path.
+with e4m3 layer GEMMs (Qwen2Encoder); the default "bf16" is the unchanged path.  ``is_causal=True`` runs the model as
+``Qwen2Model.forward(is_causal=True)`` does (causal attention in every layer, last-token pooling as before).
 """
 from __future__ import annotations
 
@@ -25,13 +26,17 @@ class GTEEmbedding(BaseEmbedding):
     _device: str = PrivateAttr()
     _embed_type: int = PrivateAttr()
     _precision: str = PrivateAttr()
+    _is_causal: bool = PrivateAttr()
 
     def __init__(self, model_name: str = None, embed_type: int = 0, encoder: Qwen2Encoder = None, tokenizer=None,
-                 device: str = "cuda", precision: str = "bf16", **kwargs: Any) -> None:
+                 device: str = "cuda", precision: str = "bf16", is_causal: bool = False, **kwargs: Any) -> None:
         _check_precision(precision)
         given = getattr(encoder, "precision", "bf16")
         if encoder is not None and given != precision:
             raise ValueError(f"precision={precision!r} but the given encoder runs {given!r}")
+        given_causal = getattr(encoder, "causal", False)
+        if encoder is not None and given_causal != bool(is_causal):
+            raise ValueError(f"is_causal={is_causal!r} but the given encoder has causal={given_causal!r}")
         if encoder is None:
             cfgd = _loading.load_config(model_name)
             cfg = Qwen2Config(vocab_size=cfgd["vocab_size"], hidden_size=cfgd["hidden_size"],
@@ -39,9 +44,10 @@ class GTEEmbedding(BaseEmbedding):
                               num_attention_heads=cfgd["num_attention_heads"],
                               num_key_value_heads=cfgd.get("num_key_value_heads", cfgd["num_attention_heads"]),
                               max_position_embeddings=min(cfgd.get("max_position_embeddings", 8192), 32768),
-                              rms_norm_eps=cfgd.get("rms_norm_eps", 1e-6), rope_theta=cfgd.get("rope_theta", 10000.0))
+                              rms_norm_eps=cfgd.get("rms_norm_eps", 1e-6), rope_theta=cfgd.get("rope_theta", 10000.0),
+                              sliding_window=cfgd.get("sliding_window"))     # the causal mask applies it (:1050)
             encoder = Qwen2Encoder(cfg, _loading.strip_prefix(_loading.load_state_dict(model_name)), device=device,
-                                   precision=precision)
+                                   precision=precision, causal=is_causal)
         if tokenizer is None:
             tokenizer = _loading.load_tokenizer(model_name)
         kwargs.setdefault("model_name", model_name or "gte-qwen2")
@@ -51,6 +57,7 @@ class GTEEmbedding(BaseEmbedding):
         self._device = str(encoder.device)
         self._embed_type = embed_type
         self._precision = precision
+        self._is_causal = bool(is_causal)
 
     def get_detailed_instruct(self, query: str) -> str:
         """gte_embeddings.py:52-53."""

@@ -45,14 +45,16 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
 
 
 def attention(qkv: torch.Tensor, cu: torch.Tensor, max_len: int, n_heads: int, n_kv: int, head_dim: int,
-              out: Optional[torch.Tensor] = None) -> torch.Tensor:
+              out: Optional[torch.Tensor] = None, causal: bool = False) -> torch.Tensor:
+    """Attention over packed q|k|v rows; ``causal=True``: row r of a sequence sees its keys 0..r (ezr_attn_causal)."""
     L = _lib.lib()
     t = qkv.shape[0]
     if out is None:
         out = torch.empty(t, n_heads * head_dim, dtype=torch.bfloat16, device=qkv.device)
-    _lib.check(L.ezr_attn_bidir(_lib.ptr(qkv), t, qkv.stride(0), _lib.ptr(cu), cu.numel() - 1, max_len, n_heads, n_kv,
+    name = "ezr_attn_causal" if causal else "ezr_attn_bidir"
+    _lib.check(getattr(L, name)(_lib.ptr(qkv), t, qkv.stride(0), _lib.ptr(cu), cu.numel() - 1, max_len, n_heads, n_kv,
                                 head_dim, 1.0 / math.sqrt(head_dim), _lib.ptr(out), out.stride(0), _lib.stream_ptr()),
-               "ezr_attn_bidir")
+               name)
     return out
 
 
@@ -225,6 +227,7 @@ class Qwen2Config:
     max_position_embeddings: int = 8192
     rms_norm_eps: float = 1e-6
     rope_theta: float = 1000000.0
+    sliding_window: Optional[int] = None    # Qwen2's causal mask window (not implemented: longer causal inputs are refused)
 
     @property
     def head_dim(self) -> int:
@@ -258,13 +261,19 @@ class Qwen2Encoder:
 
     ``precision="fp8"`` holds the layer weights as e4m3 with per-channel scales only and runs every layer GEMM on
     the e4m3 kernel (activations quantised per row); embeddings, norms, attention, RoPE, pooling and the residual
-    stream stay bf16.  Lossy: see DESIGN.md 4.5a for its error bound."""
+    stream stay bf16.  Lossy: see DESIGN.md 4.5a for its error bound.
 
-    def __init__(self, cfg: Qwen2Config, state: Dict[str, torch.Tensor], device="cuda", precision: str = "bf16"):
+    ``causal=True`` runs the stack as ``Qwen2Model.forward(is_causal=True)`` does (modeling_qwen.py:1043-1051): every
+    layer's attention lets token r of a sequence see tokens 0..r only; pooling stays last-token.  A sequence longer
+    than ``cfg.sliding_window`` is refused: the window is not implemented."""
+
+    def __init__(self, cfg: Qwen2Config, state: Dict[str, torch.Tensor], device="cuda", precision: str = "bf16",
+                 causal: bool = False):
         _check_precision(precision)
         _lib.require_cuda()
         self.cfg = cfg
         self.precision = precision
+        self.causal = bool(causal)
         self.device = torch.device(device)
         if cfg.head_dim not in (64, 128):
             raise ValueError("head_dim must be 64 or 128")
@@ -303,6 +312,9 @@ class Qwen2Encoder:
         d, hd, H, KV = cfg.hidden_size, cfg.head_dim, cfg.num_attention_heads, cfg.num_key_value_heads
         dev = self.device
         batch.check_positions(cfg.max_position_embeddings)
+        if self.causal and cfg.sliding_window is not None and batch.max_len > cfg.sliding_window:
+            raise ValueError(f"a sequence of {batch.max_len} tokens is longer than the causal sliding window of "
+                             f"{cfg.sliding_window}, which this encoder does not implement")
         with torch.cuda.device(dev):
             st = _lib.stream_ptr()
             x = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
@@ -320,7 +332,7 @@ class Qwen2Encoder:
                 gemm(xn, ly["wqkv"], bias=ly["bqkv"], out=qkv)
                 _lib.check(L.ezr_rope(_lib.ptr(qkv), qkv.stride(0), _lib.ptr(batch.positions), _lib.ptr(self.cos),
                                       _lib.ptr(self.sin), cfg.max_position_embeddings, H + KV, hd, t, st), "ezr_rope")
-                attention(qkv, batch.cu, batch.max_len, H, KV, hd, out=ao)
+                attention(qkv, batch.cu, batch.max_len, H, KV, hd, out=ao, causal=self.causal)
                 gemm(ao, ly["wo"], residual=x, out=x)
                 rmsnorm(x, ly["ln2"], cfg.rms_norm_eps, out=xn)
                 gemm(xn, ly["wgu"], out=act, epilogue=EPI_SWIGLU)
@@ -343,7 +355,7 @@ class Qwen2Encoder:
             gemm_fp8(x8, xs, *ly["wqkv"], bias=ly["bqkv"], out=qkv)
             _lib.check(L.ezr_rope(_lib.ptr(qkv), qkv.stride(0), _lib.ptr(batch.positions), _lib.ptr(self.cos),
                                   _lib.ptr(self.sin), cfg.max_position_embeddings, H + KV, hd, t, st), "ezr_rope")
-            attention(qkv, batch.cu, batch.max_len, H, KV, hd, out=ao)
+            attention(qkv, batch.cu, batch.max_len, H, KV, hd, out=ao, causal=self.causal)
             quant_rows(ao, a8, as_)
             gemm_fp8(a8, as_, *ly["wo"], residual=x, out=x)
             rmsnorm_fp8(x, ly["ln2"], cfg.rms_norm_eps, out8=x8, scale=xs)
@@ -369,12 +381,14 @@ class Qwen2Encoder:
         return out_b, out_f
 
     def flops(self, lens: Sequence[int]) -> float:
-        """SURVEY.md 8(d): layers*(4Ld^2 + 4Ld*kv_dim + 6Ld*ffn + 4L^2 d) per sequence."""
+        """SURVEY.md 8(d): layers*(4Ld^2 + 4Ld*kv_dim + 6Ld*ffn + 4L^2 d) per sequence; causal attention counts the
+        visible keys only, 2L(L+1)d instead of 4L^2 d."""
         c = self.cfg
         kvd = c.num_key_value_heads * c.head_dim
+        att = (lambda n: 2 * n * (n + 1) * c.hidden_size) if self.causal else (lambda n: 4 * n * n * c.hidden_size)
         return float(sum(c.num_hidden_layers * (4 * n * c.hidden_size ** 2 + 4 * n * c.hidden_size * kvd
                                                 + 6 * n * c.hidden_size * c.intermediate_size
-                                                + 4 * n * n * c.hidden_size) for n in lens))
+                                                + att(n)) for n in lens))
 
 
 # -------------------------------------------------------------------------------------- BERT-shaped

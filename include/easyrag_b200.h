@@ -383,9 +383,15 @@ int ezr_layernorm_fp8(const void* x, int64_t ldx, const void* gamma, const void*
 int ezr_attn_bidir(const void* qkv, int64_t n_tokens, int64_t ld, const int32_t* cu_seqlens, int32_t n_seq,
                    int32_t max_len, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, float softmax_scale, void* out,
                    int64_t ldo, void* stream);
+/* causal attention over the same packed layout, same arguments and checks: query row r of a sequence sees its keys
+ * 0..r (Qwen2Model.forward(is_causal=True) on a padding-free batch).  wgmma kernel only: under
+ * ezr_attn_set_kernel(1) it returns EZR_ERR_INVALID, the mma.sync kernel being bidirectional only. */
+int ezr_attn_causal(const void* qkv, int64_t n_tokens, int64_t ld, const int32_t* cu_seqlens, int32_t n_seq,
+                    int32_t max_len, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, float softmax_scale, void* out,
+                    int64_t ldo, void* stream);
 /* 0 = wgmma kernel (default), 1 = the warp-level mma.sync kernel (kept as an independent cross-check) */
 int ezr_attn_set_kernel(int32_t which);
-/* "wgmma" / "mma.sync": what the last ezr_attn_bidir call on this thread launched */
+/* "wgmma" / "wgmma-causal" / "mma.sync": what the last ezr_attn_bidir / ezr_attn_causal call on this thread launched */
 const char* ezr_attn_last_kernel(void);
 int ezr_embed_gather(const int32_t* ids, int32_t n_tokens, const void* table, int64_t ldt, int32_t vocab, int32_t dim,
                      void* out, int64_t ldo, void* stream);
