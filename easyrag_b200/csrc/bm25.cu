@@ -869,7 +869,9 @@ int ezr_bm25_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t*
     int rc = check_index(ix);
     if (rc) return rc;
     EZR_CHECK_ARG(k >= 1 && k <= kSelMaxK, "bm25_topk: k=%d out of [1,%d]", k, kSelMaxK);
-    EZR_CHECK_ARG(q_group == nullptr || ix->doc_group != nullptr, "bm25_topk: q_group given but index has no doc_group");
+    // an empty shard's doc_group is empty, and an empty tensor has no address: nothing is filtered, so no check
+    EZR_CHECK_ARG(q_group == nullptr || ix->doc_group != nullptr || ix->n_docs == 0,
+                  "bm25_topk: q_group given but index has no doc_group");
     if (n_queries == 0) return EZR_OK;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t need = ezr_bm25_topk_workspace(ix, n_queries, k);

@@ -203,7 +203,8 @@ int ezr_dense_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t
     EZR_CHECK_ARG(dim >= 1, "dense_topk: dim must be >= 1");
     EZR_CHECK_ARG(n_rows >= 0 && n_rows < ((int64_t)1 << 31), "dense_topk: n_rows out of range");
     EZR_CHECK_ARG(ld_corpus >= dim && ld_queries >= dim, "dense_topk: row stride smaller than dim");
-    EZR_CHECK_ARG(q_group == nullptr || doc_group != nullptr, "dense_topk: q_group without doc_group");
+    // an empty shard's doc_group is empty, and an empty tensor has no address: nothing is filtered, so no check
+    EZR_CHECK_ARG(q_group == nullptr || doc_group != nullptr || n_rows == 0, "dense_topk: q_group without doc_group");
     cudaStream_t st = (cudaStream_t)stream;
     if (n_queries == 0) return EZR_OK;
     if (n_rows == 0) {

@@ -523,11 +523,14 @@ dense_s8_rescore_kernel(const __nv_bfloat16* __restrict__ corpus, int64_t ldc, i
         sel_maybe_flush<float>(m, k);
     }
     sel_compact<float>(m, k);
+    // sel_compact pads the buffer only up to the next power of two of what it holds: the slots past the count are
+    // written here, id -1, as every top-k route leaves them (the sharded merge reads every slot with an id >= 0)
+    const int got = *m.cnt;
     for (int i = threadIdx.x; i < k; i += blockDim.x) {
-        out_scores[(int64_t)q * k + i] = m.ks[i];
-        out_ids[(int64_t)q * k + i] = m.kid[i];
+        out_scores[(int64_t)q * k + i] = i < got ? m.ks[i] : -INFINITY;
+        out_ids[(int64_t)q * k + i] = i < got ? m.kid[i] : -1;
     }
-    if (threadIdx.x == 0 && out_counts) out_counts[q] = n < k ? n : k;
+    if (threadIdx.x == 0 && out_counts) out_counts[q] = got;
 }
 
 // ------------------------------------------------------------------ host ----
@@ -603,7 +606,9 @@ int ezr_dense_s8_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int6
     EZR_CHECK_ARG(n_rows >= 0 && n_rows < ((int64_t)1 << 31), "dense_s8_topk: n_rows out of range");
     EZR_CHECK_ARG(ld_corpus >= dim && ld_queries >= dim && ld_s8 >= dim, "dense_s8_topk: row stride smaller than dim");
     EZR_CHECK_ARG(ld_corpus % 8 == 0 && ld_s8 % 16 == 0, "dense_s8_topk: row strides must be 16-byte multiples");
-    EZR_CHECK_ARG(q_group == nullptr || doc_group != nullptr, "dense_s8_topk: q_group without doc_group");
+    // an empty shard's doc_group is empty, and an empty tensor has no address: nothing is filtered, so no check
+    EZR_CHECK_ARG(q_group == nullptr || doc_group != nullptr || n_rows == 0,
+                  "dense_s8_topk: q_group without doc_group");
     EZR_CHECK_ARG(((uintptr_t)corpus_bf16 & 15) == 0 && ((uintptr_t)corpus_s8 & 15) == 0,
                   "dense_s8_topk: corpus rows must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
