@@ -103,10 +103,10 @@ SIGNATURES = {
     "ezr_profile_enable": (C.c_int, [_i32]),
     "ezr_profile_reset": (C.c_int, []),
     "ezr_profile_read": (C.c_int, [_i32, C.POINTER(C.c_double), C.POINTER(C.c_int32)]),
-    "ezr_rerank_pack_plan": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _p, _p, _i32, _i32, _i32, _p, _p, _p,
+    "ezr_rerank_pack_plan": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _i32, _i32, _i32, _p, _p, _p,
                                        C.POINTER(C.c_int64), _p]),
-    "ezr_rerank_pack_fill": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p, _i32, _p, _i32, _i32, _i32,
-                                       _p, _p, _p, _p]),
+    "ezr_rerank_pack_fill": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p, _i32, _p, _i32, _i32,
+                                       _i32, _p, _p, _p, _p]),
     "ezr_cross_pack_workspace": (_sz, [_i32, _i32]),
     "ezr_cross_pack_plan": (C.c_int, [_p, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _i32, _i32, _p, _p,
                                       C.POINTER(C.c_int64), _p, _sz, _p]),

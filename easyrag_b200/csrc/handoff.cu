@@ -9,6 +9,7 @@
 // CSR per batch) and the sep / prompt ids are device arrays; pair p = q * k + r is candidate r of query q.
 // Output is PACKED (no padding): ids[T] + cu_seqlens[P + 1] (the layout this library's encoder kernels consume;
 // a padded [32, L] view is a copy with cu as the index), plus the per-pair query_lengths of get_inputs_v2_5.
+// Both packers keep an int32 copy of cu, so their plans refuse T >= 2^31 rather than let the offsets wrap.
 #include "ezr_common.cuh"
 #include "../../include/easyrag_b200.h"
 
@@ -17,10 +18,10 @@ namespace ezr {
 struct RerankParams {
     const int32_t* cand_ids;    // [Q, k_stride] document ids in rank order (-1 padded)
     const int32_t* cand_cnt;    // [Q]
-    int n_queries, k, k_stride, id_base;
+    int n_queries, k, k_stride, id_base, n_docs;
     const int32_t* q_ptr;       // [Q + 1] into q_tok
     const int32_t* q_tok;       // query tokens WITHOUT bos
-    const int64_t* p_ptr;       // [N + 1] into p_tok
+    const int64_t* p_ptr;       // [n_docs + 1] into p_tok
     const int32_t* p_tok;
     const int32_t* sep;         // [n_sep]
     const int32_t* prompt;      // [n_prompt]
@@ -28,13 +29,18 @@ struct RerankParams {
 };
 
 // tokens of the three parts of pair p: head = bos + query (<= 3/4 max_length query tokens), body = sep + passage
-// truncated so that head + body <= max_length, tail = sep + prompt
-__device__ __forceinline__ bool pair_parts(const RerankParams& a, int p, int& doc, int& nq, int& npass) {
+// truncated so that head + body <= max_length, tail = sep + prompt.  False for a padding slot (*bad_id stays false)
+// and for an id outside [id_base, id_base + n_docs) (*bad_id set); p_ptr is read for neither.
+__device__ __forceinline__ bool pair_parts(const RerankParams& a, int p, int& doc, int& nq, int& npass,
+                                           bool* bad_id = nullptr) {
     const int q = p / a.k, r = p % a.k;
     doc = -1; nq = 0; npass = 0;
     if (r >= a.cand_cnt[q]) return false;
     doc = a.cand_ids[(int64_t)q * a.k_stride + r] - a.id_base;
-    if (doc < 0) return false;
+    if (doc < 0 || doc >= a.n_docs) {
+        if (bad_id) *bad_id = true;
+        return false;
+    }
     nq = min(a.q_ptr[q + 1] - a.q_ptr[q], a.max_length * 3 / 4);
     const int64_t plen = a.p_ptr[doc + 1] - a.p_ptr[doc];
     const int head = 1 + nq;
@@ -43,11 +49,19 @@ __device__ __forceinline__ bool pair_parts(const RerankParams& a, int p, int& do
     return true;
 }
 
-__global__ void rerank_len_kernel(const RerankParams a, int64_t* __restrict__ len, int32_t* __restrict__ query_len) {
+// per pair: the length and get_inputs_v2_5's query length (0 for padding); ids outside the passage range count
+// into *bad
+__global__ void rerank_len_kernel(const RerankParams a, int64_t* __restrict__ len, int32_t* __restrict__ query_len,
+                                  unsigned long long* __restrict__ bad) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= a.n_queries * a.k) return;
     int doc, nq, npass;
-    if (!pair_parts(a, p, doc, nq, npass)) { len[p] = 0; query_len[p] = 0; return; }
+    bool bad_id = false;
+    if (!pair_parts(a, p, doc, nq, npass, &bad_id)) {
+        len[p] = 0; query_len[p] = 0;
+        if (bad_id) atomicAdd(bad, 1ull);
+        return;
+    }
     len[p] = 1 + nq + a.n_sep + npass + a.n_sep + a.n_prompt;
     query_len[p] = 1 + nq + a.n_sep;                             // get_inputs_v2_5: len([bos] + query + sep)
 }
@@ -116,17 +130,20 @@ rerank_scan_kernel(const int64_t* __restrict__ len, int n, int64_t* __restrict__
 }
 
 static int fill_params(RerankParams& a, const int32_t* cand_ids, const int32_t* cand_cnt, int n_queries, int k, int k_stride,
-                       int id_base, const int32_t* q_ptr, const int32_t* q_tok, const int64_t* p_ptr, const int32_t* p_tok,
+                       int id_base, int n_docs, const int32_t* q_ptr, const int32_t* q_tok, const int64_t* p_ptr,
+                       const int32_t* p_tok,
                        const int32_t* sep, int n_sep, const int32_t* prompt, int n_prompt, int bos, int max_length) {
     EZR_CHECK_ARG(cand_ids && cand_cnt && q_ptr && p_ptr && (q_tok || true) && p_tok, "rerank_pack: NULL argument");
-    EZR_CHECK_ARG(n_queries >= 0 && k >= 1 && k_stride >= k, "rerank_pack: bad n_queries / k / stride");
+    EZR_CHECK_ARG(n_queries >= 0 && k >= 1 && k_stride >= k && n_docs >= 0,
+                  "rerank_pack: bad n_queries / k / stride / n_docs");
     EZR_CHECK_ARG(n_sep >= 0 && n_prompt >= 0 && (n_sep == 0 || sep) && (n_prompt == 0 || prompt) && max_length >= 8,
                   "rerank_pack: bad sep / prompt / max_length");
     EZR_CHECK_ARG((int64_t)n_queries * k < ((int64_t)1 << 30), "rerank_pack: too many pairs");
     EZR_CHECK_ARG(1 + max_length * 3 / 4 + n_sep <= max_length,
                   "rerank_pack: max_length=%d leaves no room for bos + query + sep (%d sep ids)", max_length, n_sep);
     a.cand_ids = cand_ids; a.cand_cnt = cand_cnt; a.n_queries = n_queries; a.k = k; a.k_stride = k_stride;
-    a.id_base = id_base; a.q_ptr = q_ptr; a.q_tok = q_tok; a.p_ptr = p_ptr; a.p_tok = p_tok; a.sep = sep; a.prompt = prompt;
+    a.id_base = id_base; a.n_docs = n_docs; a.q_ptr = q_ptr; a.q_tok = q_tok; a.p_ptr = p_ptr; a.p_tok = p_tok;
+    a.sep = sep; a.prompt = prompt;
     a.n_sep = n_sep; a.n_prompt = n_prompt; a.bos = bos; a.max_length = max_length;
     return EZR_OK;
 }
@@ -225,6 +242,9 @@ __global__ void cross_fill_kernel(const CrossParams a, const int64_t* __restrict
     }
 }
 
+// both packers hand the encoder int32 cu_seqlens: a batch holds fewer than 2^31 tokens
+constexpr int64_t kMaxPackTokens = (int64_t)1 << 31;
+
 static int cross_params(CrossParams& a, const int32_t* cand_ids, const int32_t* cand_cnt, int n_queries, int k,
                         int k_stride, int id_base, int n_docs, const int32_t* q_ptr, const int32_t* q_tok,
                         const int64_t* p_ptr, const int32_t* p_tok, int cls, int sep, int n_mid, int type_b,
@@ -297,6 +317,8 @@ int ezr_cross_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32_
     const int32_t n_bad = *reinterpret_cast<const int32_t*>(h + 2);
     EZR_CHECK_ARG(n_bad == 0, "cross_pack_plan: %d candidate ids outside [id_base, id_base + n_docs) = [%d, %lld)", n_bad,
                   id_base, (long long)id_base + n_docs);
+    EZR_CHECK_ARG(h[0] < kMaxPackTokens, "cross_pack_plan: T=%lld tokens in %lld pairs; the int32 cu_seqlens hold fewer "
+                  "than 2^31 (split the queries)", (long long)h[0], (long long)h[1]);
     totals_host[0] = h[0];
     totals_host[1] = h[1];
     return EZR_OK;
@@ -321,11 +343,11 @@ int ezr_cross_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32_
 }
 
 int ezr_rerank_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k, int32_t k_stride,
-                         int32_t id_base, const int32_t* q_ptr, const int64_t* p_ptr, int32_t n_sep, int32_t n_prompt,
-                         int32_t max_length, int64_t* out_len, int64_t* out_cu, int32_t* out_query_len,
-                         int64_t* total_host, void* stream) {
+                         int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int64_t* p_ptr, int32_t n_sep,
+                         int32_t n_prompt, int32_t max_length, int64_t* out_len, int64_t* out_cu,
+                         int32_t* out_query_len, int64_t* total_host, void* stream) {
     RerankParams a;
-    int rc = fill_params(a, cand_ids, cand_cnt, n_queries, k, k_stride, id_base, q_ptr, nullptr, p_ptr,
+    int rc = fill_params(a, cand_ids, cand_cnt, n_queries, k, k_stride, id_base, n_docs, q_ptr, nullptr, p_ptr,
                          reinterpret_cast<const int32_t*>(1), n_sep ? reinterpret_cast<const int32_t*>(1) : nullptr, n_sep,
                          n_prompt ? reinterpret_cast<const int32_t*>(1) : nullptr, n_prompt, 0, max_length);
     if (rc) return rc;
@@ -333,23 +355,33 @@ int ezr_rerank_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32
     cudaStream_t st = (cudaStream_t)stream;
     const int n_pairs = n_queries * k;
     if (n_pairs == 0) { *total_host = 0; return EZR_OK; }
-    rerank_len_kernel<<<ceil_div(n_pairs, 256), 256, 0, st>>>(a, out_len, out_query_len);
+    // out_cu[0] counts the bad ids until the scan writes its 0; the count is copied out before that, in stream order
+    unsigned long long* bad = reinterpret_cast<unsigned long long*>(out_cu);
+    EZR_CUDA(cudaMemsetAsync(bad, 0, 8, st));
+    rerank_len_kernel<<<ceil_div(n_pairs, 256), 256, 0, st>>>(a, out_len, out_query_len, bad);
     EZR_LAUNCH_CHECK();
+    int64_t h[2] = {0, 0};
+    EZR_CUDA(cudaMemcpyAsync(h, bad, 8, cudaMemcpyDeviceToHost, st));
     rerank_scan_kernel<<<1, 1024, 0, st>>>(out_len, n_pairs, out_cu);
     EZR_LAUNCH_CHECK();
-    EZR_CUDA(cudaMemcpyAsync(total_host, out_cu + n_pairs, 8, cudaMemcpyDeviceToHost, st));
+    EZR_CUDA(cudaMemcpyAsync(h + 1, out_cu + n_pairs, 8, cudaMemcpyDeviceToHost, st));
     EZR_CUDA(cudaStreamSynchronize(st));
+    EZR_CHECK_ARG(h[0] == 0, "rerank_pack_plan: %lld candidate ids outside [id_base, id_base + n_docs) = [%d, %lld)",
+                  (long long)h[0], id_base, (long long)id_base + n_docs);
+    EZR_CHECK_ARG(h[1] < kMaxPackTokens, "rerank_pack_plan: T=%lld tokens in %d pairs; the int32 cu_seqlens hold fewer "
+                  "than 2^31 (split the queries)", (long long)h[1], n_pairs);
+    *total_host = h[1];
     return EZR_OK;
 }
 
 int ezr_rerank_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k, int32_t k_stride,
-                         int32_t id_base, const int32_t* q_ptr, const int32_t* q_tok, const int64_t* p_ptr,
+                         int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int32_t* q_tok, const int64_t* p_ptr,
                          const int32_t* p_tok, const int32_t* sep, int32_t n_sep, const int32_t* prompt, int32_t n_prompt,
                          int32_t bos, int32_t max_length, const int64_t* cu, int32_t* out_ids, int32_t* out_cu32,
                          void* stream) {
     RerankParams a;
-    int rc = fill_params(a, cand_ids, cand_cnt, n_queries, k, k_stride, id_base, q_ptr, q_tok, p_ptr, p_tok, sep, n_sep,
-                         prompt, n_prompt, bos, max_length);
+    int rc = fill_params(a, cand_ids, cand_cnt, n_queries, k, k_stride, id_base, n_docs, q_ptr, q_tok, p_ptr, p_tok, sep,
+                         n_sep, prompt, n_prompt, bos, max_length);
     if (rc) return rc;
     EZR_CHECK_ARG(cu && out_ids && out_cu32 && q_tok, "rerank_pack_fill: NULL argument");
     cudaStream_t st = (cudaStream_t)stream;

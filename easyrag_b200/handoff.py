@@ -93,6 +93,7 @@ class RerankPacker:
         for t in passage_tokens:
             ptr.append(ptr[-1] + len(t))
         flat = [int(x) for t in passage_tokens for x in t]
+        self.n_docs = len(ptr) - 1
         self.p_ptr = torch.tensor(ptr, dtype=torch.int64, device=self.device)
         self.p_tok = torch.tensor(flat if flat else [0], dtype=torch.int32, device=self.device)
         self.sep = torch.tensor(list(sep) or [0], dtype=torch.int32, device=self.device)
@@ -103,7 +104,9 @@ class RerankPacker:
     def pack(self, cand_ids: torch.Tensor, cand_counts: torch.Tensor, q_ptr: torch.Tensor, q_tok: torch.Tensor,
              stream=None) -> PackedRerankInput:
         """``cand_ids`` int32 [Q, k] / ``cand_counts`` int32 [Q]: a ``TopK`` of the coarse ranker (device tensors);
-        ``q_ptr`` int32 [Q+1] / ``q_tok`` int32: the batch's query ids (CSR, without bos)."""
+        ``q_ptr`` int32 [Q+1] / ``q_tok`` int32: the batch's query ids (CSR, without bos).  Raises before any token
+        buffer is allocated if a candidate id inside a query's count lies outside
+        ``[id_base, id_base + len(passage_tokens))``, or if the pack would hold 2^31 tokens or more."""
         import ctypes
         L = _lib.lib()
         dev = self.device
@@ -123,16 +126,17 @@ class RerankPacker:
         st = _lib.stream_ptr(stream)
         with torch.cuda.device(dev):
             _lib.check(L.ezr_rerank_pack_plan(_lib.ptr(ids), _lib.ptr(cnt), nq, k, ids.stride(0), self.id_base,
-                                              _lib.ptr(qp), _lib.ptr(self.p_ptr), self.n_sep, self.n_prompt,
-                                              self.max_length, _lib.ptr(ln), _lib.ptr(cu64), _lib.ptr(qlen),
-                                              ctypes.byref(total), st), "ezr_rerank_pack_plan")
+                                              self.n_docs, _lib.ptr(qp), _lib.ptr(self.p_ptr), self.n_sep,
+                                              self.n_prompt, self.max_length, _lib.ptr(ln), _lib.ptr(cu64),
+                                              _lib.ptr(qlen), ctypes.byref(total), st), "ezr_rerank_pack_plan")
             out = torch.empty(max(int(total.value), 1), dtype=torch.int32, device=dev)
             cu32 = torch.zeros(n_pairs + 1, dtype=torch.int32, device=dev)
             if n_pairs:
                 _lib.check(L.ezr_rerank_pack_fill(_lib.ptr(ids), _lib.ptr(cnt), nq, k, ids.stride(0), self.id_base,
-                                                  _lib.ptr(qp), _lib.ptr(qt), _lib.ptr(self.p_ptr), _lib.ptr(self.p_tok),
-                                                  _lib.ptr(self.sep), self.n_sep, _lib.ptr(self.prompt), self.n_prompt,
-                                                  self.bos, self.max_length, _lib.ptr(cu64), _lib.ptr(out),
-                                                  _lib.ptr(cu32), st), "ezr_rerank_pack_fill")
+                                                  self.n_docs, _lib.ptr(qp), _lib.ptr(qt), _lib.ptr(self.p_ptr),
+                                                  _lib.ptr(self.p_tok), _lib.ptr(self.sep), self.n_sep,
+                                                  _lib.ptr(self.prompt), self.n_prompt, self.bos, self.max_length,
+                                                  _lib.ptr(cu64), _lib.ptr(out), _lib.ptr(cu32), st),
+                           "ezr_rerank_pack_fill")
         return PackedRerankInput(ids=out[:int(total.value)], cu=cu32, query_len=qlen[:n_pairs],
                                  prompt_len=self.n_sep + self.n_prompt, n_queries=nq, k=k)

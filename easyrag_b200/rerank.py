@@ -29,6 +29,7 @@ from .schema import BaseNodePostprocessor, Field, MetadataMode, NodeWithScore, P
 DEFAULT_SENTENCE_TRANSFORMER_MAX_LENGTH = 512
 DEFAULT_MAX_TOKENS = 65536
 MAX_CANDIDATES = 1024          # candidates per query the ordering kernel holds (one CTA per query)
+MAX_CHUNK_PAIRS = 65535        # sequences one attention launch takes (its grid's y extent)
 
 # family -> (separators between the two segments, token type of the second segment); see ezr_cross_pack_plan
 _TEMPLATES = {"bert": (1, 1), "roberta": (2, 0)}
@@ -233,11 +234,12 @@ class CrossEncoderReranker:
         return out, all_scores
 
     def chunks(self, cu_h: np.ndarray) -> List[Tuple[int, int]]:
-        """Consecutive runs [p0, p1) of whole pairs holding at most ``max_tokens`` tokens each."""
+        """Consecutive runs [p0, p1) of whole pairs holding at most ``max_tokens`` tokens and at most
+        ``MAX_CHUNK_PAIRS`` pairs each."""
         out, p0, n = [], 0, cu_h.size - 1
         while p0 < n:
             p1 = int(np.searchsorted(cu_h, cu_h[p0] + self.max_tokens, side="right")) - 1
-            p1 = min(max(p1, p0 + 1), n)
+            p1 = min(max(p1, p0 + 1), n, p0 + MAX_CHUNK_PAIRS)
             out.append((p0, p1))
             p0 = p1
         return out

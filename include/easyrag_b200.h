@@ -286,15 +286,16 @@ int ezr_fuse_lists(int32_t rrf, int32_t n_lists, const int32_t* const* ids_host,
  * get_inputs_v2_5, sliced 32 at a time by _postprocess_nodes :309-322), built on the device.  Pair p = q*k + r is
  * candidate r of query q: [bos] + query[: 3/4 max_length] + sep + passage (the pair truncated to max_length, the
  * passage gives way) + sep + prompt.  Queries ("A: ..." ids, q_ptr/q_tok) and passages ("B: ..." ids of every chunk,
- * tokenised once at index time, p_ptr/p_tok) are device CSR arrays.  Output is packed: ids[T], cu[P+1]; pairs past a
- * query's count are empty.  plan: lengths, their scan (int64) and get_inputs_v2_5's query_lengths; *total_host = T
- * (synchronises).  fill: the tokens + an int32 copy of cu (the cu_seqlens format of the encoder kernels). */
+ * tokenised once at index time, n_docs of them, ids id_base ..., p_ptr/p_tok) are device CSR arrays.  Output is packed:
+ * ids[T], cu[P+1]; pairs past a query's count are empty.  plan: lengths, their scan (int64) and get_inputs_v2_5's
+ * query_lengths; *total_host = T (synchronises; a candidate id outside the passage range, or T >= 2^31, is
+ * EZR_ERR_INVALID).  fill: the tokens + an int32 copy of cu (the cu_seqlens format of the encoder kernels). */
 int ezr_rerank_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k, int32_t k_stride,
-                         int32_t id_base, const int32_t* q_ptr, const int64_t* p_ptr, int32_t n_sep, int32_t n_prompt,
-                         int32_t max_length, int64_t* out_len, int64_t* out_cu, int32_t* out_query_len,
-                         int64_t* total_host, void* stream);
+                         int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int64_t* p_ptr, int32_t n_sep,
+                         int32_t n_prompt, int32_t max_length, int64_t* out_len, int64_t* out_cu,
+                         int32_t* out_query_len, int64_t* total_host, void* stream);
 int ezr_rerank_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k, int32_t k_stride,
-                         int32_t id_base, const int32_t* q_ptr, const int32_t* q_tok, const int64_t* p_ptr,
+                         int32_t id_base, int32_t n_docs, const int32_t* q_ptr, const int32_t* q_tok, const int64_t* p_ptr,
                          const int32_t* p_tok, const int32_t* sep, int32_t n_sep, const int32_t* prompt, int32_t n_prompt,
                          int32_t bos, int32_t max_length, const int64_t* cu, int32_t* out_ids, int32_t* out_cu32,
                          void* stream);
@@ -310,7 +311,7 @@ int ezr_rerank_pack_fill(const int32_t* cand_ids, const int32_t* cand_cnt, int32
  * n_docs of them, ids id_base ...) are device CSR arrays of ids tokenised without special tokens.
  * Only the real pairs (candidate r < counts[q]) are packed: pair pair_off[q] + r, P = pair_off[Q] in all.
  * plan: pair_off int32 [Q + 1], cu int32 [P + 1] (the caller sizes it Q * k + 1), totals_host = {T, P}
- *       (synchronises; a candidate id outside the passage range is EZR_ERR_INVALID).
+ *       (synchronises; a candidate id outside the passage range, or T >= 2^31, is EZR_ERR_INVALID).
  * fill: ids / types / positions int32 [T], reading the plan's workspace. */
 size_t ezr_cross_pack_workspace(int32_t n_queries, int32_t k);
 int ezr_cross_pack_plan(const int32_t* cand_ids, const int32_t* cand_cnt, int32_t n_queries, int32_t k,

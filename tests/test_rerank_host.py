@@ -118,6 +118,16 @@ def test_chunks_hold_whole_pairs_under_the_budget():
     assert len(rerank.CrossEncoderReranker.chunks(SimpleNamespace(max_tokens=10 ** 9), cu)) == 1
 
 
+def test_chunks_stay_within_the_attention_sequence_limit():
+    """Many short pairs under a large budget: a chunk holds at most MAX_CHUNK_PAIRS pairs, the sequences one attention
+    launch takes."""
+    cu = np.arange(0, 3 * 20 * rerank.MAX_CHUNK_PAIRS + 1, 20, dtype=np.int64)          # 3 * MAX_CHUNK_PAIRS pairs
+    parts = rerank.CrossEncoderReranker.chunks(SimpleNamespace(max_tokens=1 << 22), cu)
+    assert parts == [(i * rerank.MAX_CHUNK_PAIRS, (i + 1) * rerank.MAX_CHUNK_PAIRS) for i in range(3)]
+    parts = rerank.CrossEncoderReranker.chunks(SimpleNamespace(max_tokens=20 * 1000), cu)
+    assert all(p1 - p0 == 1000 for p0, p1 in parts[:-1])
+
+
 def test_model_rejects_multi_label_heads_and_unsupported_head_dims():
     cfg = BertConfig(vocab_size=50, hidden_size=128, intermediate_size=256, num_hidden_layers=1,
                      num_attention_heads=2, max_position_embeddings=64)
