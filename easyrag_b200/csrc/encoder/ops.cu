@@ -8,15 +8,9 @@
 //   rotary embedding        modeling_qwen.py:137-169 half-split layout, cos/sin tables cast to bf16, bf16 products
 //   last_token_pool + F.normalize(p=2) in bf16       gte_embeddings.py:42-50,70
 //   BERT embeddings + LayerNorm, CLS / mean pooling, fp32 normalise   (SentenceTransformer.encode, hf_embeddings.py:118-123)
-#include "../ezr_common.cuh"
+#include "norm_row.cuh"
 
 namespace ezr {
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // block-wide sum for blockDim.x <= 1024 (result broadcast to all threads)
 __device__ __forceinline__ float block_sum(float v, float* sh) {
@@ -126,69 +120,15 @@ __global__ void norm_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, co
     }
 }
 
-// Warp-per-row variant for dim % 8 == 0 and dim <= 256 * MAXC: the row lives in registers (MAXC 16-byte chunks per
-// lane), statistics by warp shuffles only, 8 rows per 256-thread CTA.  Same rounding points as norm_kernel.
+// Warp-per-row variant for dim % 8 == 0 and dim <= 256 * MAXC (norm_row_warp), 8 rows per 256-thread CTA.
 template <int MODE, int MAXC>
 __global__ void __launch_bounds__(256)
 norm_warp_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, const __nv_bfloat16* __restrict__ gamma,
                  const __nv_bfloat16* __restrict__ beta, float eps, int dim, __nv_bfloat16* __restrict__ out,
                  int64_t ldo, int n_rows) {
-    const int lane = threadIdx.x & 31;
-    const int r = blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (r >= n_rows) return;
-    const int n_chunks = dim >> 3;
-    const uint4* xr = reinterpret_cast<const uint4*>(x + (int64_t)r * ldx);
     float v[MAXC][8];
-    float s = 0.f, q = 0.f;
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-        const int ci = lane + c * 32;
-        if (ci < n_chunks) {
-            const uint4 u = __ldg(xr + ci);
-            const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(&u);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { v[c][j] = __bfloat162float(h[j]); s += v[c][j]; q += v[c][j] * v[c][j]; }
-        }
-    }
-    float mean = 0.f, rstd;
-    if (MODE == 0) {
-        rstd = rsqrtf(warp_sum(q) / dim + eps);
-    } else {
-        mean = warp_sum(s) / dim;
-        float q2 = 0.f;
-#pragma unroll
-        for (int c = 0; c < MAXC; ++c) {
-            if (lane + c * 32 < n_chunks) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) { const float d = v[c][j] - mean; q2 += d * d; }
-            }
-        }
-        rstd = rsqrtf(warp_sum(q2) / dim + eps);
-    }
-    uint4* orow = reinterpret_cast<uint4*>(out + (int64_t)r * ldo);
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-        const int ci = lane + c * 32;
-        if (ci < n_chunks) {
-            const uint4 g4 = __ldg(reinterpret_cast<const uint4*>(gamma) + ci);
-            const __nv_bfloat16* gh = reinterpret_cast<const __nv_bfloat16*>(&g4);
-            uint4 b4 = make_uint4(0u, 0u, 0u, 0u);
-            if (MODE == 1) b4 = __ldg(reinterpret_cast<const uint4*>(beta) + ci);
-            const __nv_bfloat16* bh = reinterpret_cast<const __nv_bfloat16*>(&b4);
-            uint4 o4;
-            __nv_bfloat16* oh = reinterpret_cast<__nv_bfloat16*>(&o4);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                if (MODE == 0) {
-                    const float y = __bfloat162float(__float2bfloat16(v[c][j] * rstd));      // .to(input_dtype)
-                    oh[j] = __float2bfloat16(__bfloat162float(gh[j]) * y);
-                } else {
-                    oh[j] = __float2bfloat16((v[c][j] - mean) * rstd * __bfloat162float(gh[j]) + __bfloat162float(bh[j]));
-                }
-            }
-            orow[ci] = o4;
-        }
-    }
+    norm_row_warp<MODE, MAXC>(x, ldx, gamma, beta, eps, dim, blockIdx.x * 8 + (threadIdx.x >> 5), n_rows, true, out,
+                              ldo, v);
 }
 
 template <int MODE>

@@ -7,24 +7,13 @@
 // the conversion (cvt.rn.satfinite.e4m3x2.f32) rounds to nearest-even without ever saturating; the result equals
 // torch's (x.float() / s).to(torch.float8_e4m3fn) bit for bit.
 //
-// The fused norms compute exactly the bf16 row of ops.cu's warp-per-row norm kernels (same statistics, same rounding
-// points), optionally store it, and quantise that bf16 row from registers: the GEMM that follows a norm reads e4m3
-// without a bf16 round trip through memory.
+// The fused norms run the row body of ops.cu's warp-per-row norm kernels (norm_row.cuh), so their bf16 row is that
+// kernel's row bit for bit; they optionally store it and quantise it from registers: the GEMM that follows a norm
+// reads e4m3 without a bf16 round trip through memory.
 #include <cuda_fp8.h>
-#include "../ezr_common.cuh"
+#include "norm_row.cuh"
 
 namespace ezr {
-
-__device__ __forceinline__ float warp_max_f8(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ float warp_sum_f8(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // The row's scale exponent e (s = 2^e) and two factors whose product is 2^-e, each a normal fp32 power of two, so
 // (x * m1) * m2 is exact: e ranges over [-141, 119] (bf16 amax from 2^-133 to below 2^128).
@@ -75,7 +64,7 @@ quant_rows_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, int rows
 #pragma unroll
         for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(__bfloat162float(h[j])));
     }
-    const Pow2Scale s = pow2_scale(warp_max_f8(amax));
+    const Pow2Scale s = pow2_scale(warp_max(amax));
     for (int i = lane; i < n8; i += 32) {
         const uint4 u = __ldg(xr + i);
         const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(&u);
@@ -87,7 +76,8 @@ quant_rows_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, int rows
     if (lane == 0) scale[r] = ldexpf(1.f, s.e);
 }
 
-// MODE 0: Qwen2RMSNorm, MODE 1: LayerNorm -- the arithmetic of norm_warp_kernel (ops.cu), then the row quantised.
+// MODE 0: Qwen2RMSNorm, MODE 1: LayerNorm -- norm_warp_kernel's row (norm_row_warp), stored to out unless it is
+// null, then quantised from registers with the absmax norm_row_warp returns.
 template <int MODE, int MAXC>
 __global__ void __launch_bounds__(256)
 norm_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, const __nv_bfloat16* __restrict__ gamma,
@@ -96,62 +86,10 @@ norm_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, const __nv_bfl
     const int lane = threadIdx.x & 31;
     const int r = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (r >= n_rows) return;
-    const int n_chunks = dim >> 3;
-    const uint4* xr = reinterpret_cast<const uint4*>(x + (int64_t)r * ldx);
     float v[MAXC][8];
-    float s = 0.f, q = 0.f;
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-        const int ci = lane + c * 32;
-        if (ci < n_chunks) {
-            const uint4 u = __ldg(xr + ci);
-            const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(&u);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { v[c][j] = __bfloat162float(h[j]); s += v[c][j]; q += v[c][j] * v[c][j]; }
-        }
-    }
-    float mean = 0.f, rstd;
-    if (MODE == 0) {
-        rstd = rsqrtf(warp_sum_f8(q) / dim + eps);
-    } else {
-        mean = warp_sum_f8(s) / dim;
-        float q2 = 0.f;
-#pragma unroll
-        for (int c = 0; c < MAXC; ++c) {
-            if (lane + c * 32 < n_chunks) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) { const float d = v[c][j] - mean; q2 += d * d; }
-            }
-        }
-        rstd = rsqrtf(warp_sum_f8(q2) / dim + eps);
-    }
-    float amax = 0.f;
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-        const int ci = lane + c * 32;
-        if (ci < n_chunks) {
-            const uint4 g4 = __ldg(reinterpret_cast<const uint4*>(gamma) + ci);
-            const __nv_bfloat16* gh = reinterpret_cast<const __nv_bfloat16*>(&g4);
-            uint4 b4 = make_uint4(0u, 0u, 0u, 0u);
-            if (MODE == 1) b4 = __ldg(reinterpret_cast<const uint4*>(beta) + ci);
-            const __nv_bfloat16* bh = reinterpret_cast<const __nv_bfloat16*>(&b4);
-            uint4 o4;
-            __nv_bfloat16* oh = reinterpret_cast<__nv_bfloat16*>(&o4);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                if (MODE == 0) {
-                    const float y = __bfloat162float(__float2bfloat16(v[c][j] * rstd));      // .to(input_dtype)
-                    oh[j] = __float2bfloat16(__bfloat162float(gh[j]) * y);
-                } else {
-                    oh[j] = __float2bfloat16((v[c][j] - mean) * rstd * __bfloat162float(gh[j]) + __bfloat162float(bh[j]));
-                }
-                v[c][j] = __bfloat162float(oh[j]);                                       // the bf16 row, kept
-                amax = fmaxf(amax, fabsf(v[c][j]));
-            }
-            if (out) reinterpret_cast<uint4*>(out + (int64_t)r * ldo)[ci] = o4;
-        }
-    }
-    const Pow2Scale sc = pow2_scale(warp_max_f8(amax));
+    const float amax = norm_row_warp<MODE, MAXC>(x, ldx, gamma, beta, eps, dim, r, n_rows, out != nullptr, out, ldo, v);
+    const int n_chunks = dim >> 3;
+    const Pow2Scale sc = pow2_scale(warp_max(amax));
     uint2* qrow = reinterpret_cast<uint2*>(out8 + (int64_t)r * ldq);
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {

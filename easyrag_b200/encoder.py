@@ -145,6 +145,26 @@ def layernorm_fp8(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps:
     return out8, scale
 
 
+# One layer loop per encoder serves both precisions.  A GEMM operand is a bf16 tensor, or an (e4m3, float32 scales)
+# pair in fp8 mode; ``q`` is the pair of buffers an operand is quantised into, None in bf16 mode.
+def _linear(a, w, **kw) -> torch.Tensor:
+    """gemm, or gemm_fp8 for a weight ``_weight`` stored as (e4m3, scales)."""
+    return gemm_fp8(*a, *w, **kw) if isinstance(w, tuple) else gemm(a, w, **kw)
+
+
+def _operand(x: torch.Tensor, q):
+    """bf16 ``x`` as a GEMM operand: itself, or quantised per row into ``q``."""
+    return x if q is None else quant_rows(x, *q)
+
+
+def _norm(x: torch.Tensor, gamma: torch.Tensor, beta: Optional[torch.Tensor], eps: float, out, q):
+    """RMSNorm (``beta`` None) or LayerNorm of ``x`` as a GEMM operand: the bf16 row written to ``out``, or quantised
+    into ``q`` by the same kernel, which then also writes the bf16 row to ``out`` unless it is None."""
+    if q is None:
+        return rmsnorm(x, gamma, eps, out=out) if beta is None else layernorm(x, gamma, beta, eps, out=out)
+    return rmsnorm_fp8(x, gamma, eps, *q, out=out) if beta is None else layernorm_fp8(x, gamma, beta, eps, *q, out=out)
+
+
 PRECISIONS = ("bf16", "fp8")
 
 
@@ -159,6 +179,21 @@ def _dest(out_bf16: Optional[torch.Tensor], n: int, d: int, device) -> torch.Ten
     if out_bf16.shape != (n, d) or out_bf16.dtype != torch.bfloat16 or not out_bf16.is_contiguous():
         raise ValueError("out_bf16 must be a contiguous bf16 [n_seq, dim] tensor (a row slice of the corpus matrix)")
     return out_bf16
+
+
+def _pool(enc, batch: PackedBatch, out_bf16: Optional[torch.Tensor], pool: int, gamma: Optional[torch.Tensor],
+          eps: float, l2: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``enc.hidden(batch)`` pooled per sequence, RMS-normed with ``gamma`` unless it is None, and L2-normalised in
+    mode ``l2`` (ezr_pool_normalize) -> (bf16 [B, d], float32 copy)."""
+    x = enc.hidden(batch)
+    d = enc.cfg.hidden_size
+    out_b = _dest(out_bf16, batch.n_seq, d, enc.device)
+    out_f = torch.empty(batch.n_seq, d, dtype=torch.float32, device=enc.device)
+    with torch.cuda.device(enc.device):
+        _lib.check(_lib.lib().ezr_pool_normalize(_lib.ptr(x), x.stride(0), _lib.ptr(batch.cu), batch.n_seq, pool,
+                                                 int(gamma is not None), _lib.ptr(gamma), eps, l2, d, _lib.ptr(out_b),
+                                                 _lib.ptr(out_f), _lib.stream_ptr()), "ezr_pool_normalize")
+    return out_b, out_f
 
 
 # ------------------------------------------------------------------------------------- packing
@@ -320,48 +355,21 @@ class Qwen2Encoder:
             x = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
             _lib.check(L.ezr_embed_gather(_lib.ptr(batch.ids), t, _lib.ptr(self.embed), self.embed.stride(0),
                                           cfg.vocab_size, d, _lib.ptr(x), x.stride(0), st), "ezr_embed_gather")
-            xn = torch.empty_like(x)
+            fp8 = self.precision == "fp8"
+            xn = None if fp8 else torch.empty_like(x)         # fp8: the norms write only their e4m3 row
             qkv = torch.empty(t, (H + 2 * KV) * hd, dtype=torch.bfloat16, device=dev)
             ao = torch.empty(t, H * hd, dtype=torch.bfloat16, device=dev)
             act = torch.empty(t, cfg.intermediate_size, dtype=torch.bfloat16, device=dev)
-            if self.precision == "fp8":
-                self._layers_fp8(batch, x, qkv, ao, act)
-                return x
+            x8, a8, act8 = (_fp8_dest(b, None, None) if fp8 else None for b in (x, ao, act))
             for ly in self.layers:
-                rmsnorm(x, ly["ln1"], cfg.rms_norm_eps, out=xn)
-                gemm(xn, ly["wqkv"], bias=ly["bqkv"], out=qkv)
+                _linear(_norm(x, ly["ln1"], None, cfg.rms_norm_eps, xn, x8), ly["wqkv"], bias=ly["bqkv"], out=qkv)
                 _lib.check(L.ezr_rope(_lib.ptr(qkv), qkv.stride(0), _lib.ptr(batch.positions), _lib.ptr(self.cos),
                                       _lib.ptr(self.sin), cfg.max_position_embeddings, H + KV, hd, t, st), "ezr_rope")
                 attention(qkv, batch.cu, batch.max_len, H, KV, hd, out=ao, causal=self.causal)
-                gemm(ao, ly["wo"], residual=x, out=x)
-                rmsnorm(x, ly["ln2"], cfg.rms_norm_eps, out=xn)
-                gemm(xn, ly["wgu"], out=act, epilogue=EPI_SWIGLU)
-                gemm(act, ly["wdown"], residual=x, out=x)
+                _linear(_operand(ao, a8), ly["wo"], residual=x, out=x)
+                _linear(_norm(x, ly["ln2"], None, cfg.rms_norm_eps, xn, x8), ly["wgu"], out=act, epilogue=EPI_SWIGLU)
+                _linear(_operand(act, act8), ly["wdown"], residual=x, out=x)
         return x
-
-    def _layers_fp8(self, batch: PackedBatch, x, qkv, ao, act) -> None:
-        """The layer loop of ``hidden`` on the e4m3 GEMMs: the norms quantise their bf16 output in the same kernel, the
-        attention output and the SwiGLU output are quantised per row before o_proj / down_proj."""
-        L = _lib.lib()
-        cfg = self.cfg
-        t = x.shape[0]
-        H, KV, hd = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        st = _lib.stream_ptr()
-        x8, xs = _fp8_dest(x, None, None)
-        a8, as_ = _fp8_dest(ao, None, None)
-        act8, acts = _fp8_dest(act, None, None)
-        for ly in self.layers:
-            rmsnorm_fp8(x, ly["ln1"], cfg.rms_norm_eps, out8=x8, scale=xs)
-            gemm_fp8(x8, xs, *ly["wqkv"], bias=ly["bqkv"], out=qkv)
-            _lib.check(L.ezr_rope(_lib.ptr(qkv), qkv.stride(0), _lib.ptr(batch.positions), _lib.ptr(self.cos),
-                                  _lib.ptr(self.sin), cfg.max_position_embeddings, H + KV, hd, t, st), "ezr_rope")
-            attention(qkv, batch.cu, batch.max_len, H, KV, hd, out=ao, causal=self.causal)
-            quant_rows(ao, a8, as_)
-            gemm_fp8(a8, as_, *ly["wo"], residual=x, out=x)
-            rmsnorm_fp8(x, ly["ln2"], cfg.rms_norm_eps, out8=x8, scale=xs)
-            gemm_fp8(x8, xs, *ly["wgu"], out=act, epilogue=EPI_SWIGLU)
-            quant_rows(act, act8, acts)
-            gemm_fp8(act8, acts, *ly["wdown"], residual=x, out=x)
 
     @torch.no_grad()
     def embed_packed(self, batch: PackedBatch, out_bf16: Optional[torch.Tensor] = None
@@ -369,16 +377,7 @@ class Qwen2Encoder:
         """-> (bf16 [B, d] unit rows for the dense index, float32 copy the embedding API returns).
         ``out_bf16``: a contiguous [B, d] bf16 destination, e.g. ``DenseIndex.rows_for_append(B)`` -- the pooling
         kernel then writes the corpus rows in place."""
-        L = _lib.lib()
-        x = self.hidden(batch)
-        d = self.cfg.hidden_size
-        out_b = _dest(out_bf16, batch.n_seq, d, self.device)
-        out_f = torch.empty(batch.n_seq, d, dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(L.ezr_pool_normalize(_lib.ptr(x), x.stride(0), _lib.ptr(batch.cu), batch.n_seq, POOL_LAST, 1,
-                                            _lib.ptr(self.norm), self.cfg.rms_norm_eps, 1, d, _lib.ptr(out_b),
-                                            _lib.ptr(out_f), _lib.stream_ptr()), "ezr_pool_normalize")
-        return out_b, out_f
+        return _pool(self, batch, out_bf16, POOL_LAST, self.norm, self.cfg.rms_norm_eps, 1)
 
     def flops(self, lens: Sequence[int]) -> float:
         """SURVEY.md 8(d): layers*(4Ld^2 + 4Ld*kv_dim + 6Ld*ffn + 4L^2 d) per sequence; causal attention counts the
@@ -477,51 +476,23 @@ class BertEncoder:
             ao = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
             y = torch.empty(t, d, dtype=torch.bfloat16, device=dev)
             act = torch.empty(t, cfg.intermediate_size, dtype=torch.bfloat16, device=dev)
-            if self.precision == "fp8":
-                self._layers_fp8(batch, x, qkv, ao, y, act)
-                return x
+            x8, a8, act8 = (_fp8_dest(b, None, None) if self.precision == "fp8" else None for b in (x, ao, act))
+            h = _operand(x, x8)
             for ly in self.layers:
-                gemm(x, ly["wqkv"], bias=ly["bqkv"], out=qkv)
+                # x, the bf16 residual stream, is written by every LayerNorm; h is x as the next GEMM's operand
+                _linear(h, ly["wqkv"], bias=ly["bqkv"], out=qkv)
                 attention(qkv, batch.cu, batch.max_len, H, H, hd, out=ao)
-                gemm(ao, ly["wo"], bias=ly["bo"], residual=x, out=y)
-                layernorm(y, ly["ln1g"], ly["ln1b"], cfg.layer_norm_eps, out=x)
-                gemm(x, ly["w1"], bias=ly["b1"], out=act, epilogue=EPI_GELU)
-                gemm(act, ly["w2"], bias=ly["b2"], residual=x, out=y)
-                layernorm(y, ly["ln2g"], ly["ln2b"], cfg.layer_norm_eps, out=x)
+                _linear(_operand(ao, a8), ly["wo"], bias=ly["bo"], residual=x, out=y)
+                h = _norm(y, ly["ln1g"], ly["ln1b"], cfg.layer_norm_eps, x, x8)
+                _linear(h, ly["w1"], bias=ly["b1"], out=act, epilogue=EPI_GELU)
+                _linear(_operand(act, act8), ly["w2"], bias=ly["b2"], residual=x, out=y)
+                h = _norm(y, ly["ln2g"], ly["ln2b"], cfg.layer_norm_eps, x, x8)
         return x
-
-    def _layers_fp8(self, batch: PackedBatch, x, qkv, ao, y, act) -> None:
-        """The layer loop of ``hidden`` on the e4m3 GEMMs.  x (bf16, the residual stream) and its e4m3 copy x8 come
-        out of the same LayerNorm kernel; the attention and GELU outputs are quantised per row."""
-        cfg = self.cfg
-        H, hd = cfg.num_attention_heads, cfg.head_dim
-        x8, xs = quant_rows(x)
-        a8, as_ = _fp8_dest(ao, None, None)
-        act8, acts = _fp8_dest(act, None, None)
-        for ly in self.layers:
-            gemm_fp8(x8, xs, *ly["wqkv"], bias=ly["bqkv"], out=qkv)
-            attention(qkv, batch.cu, batch.max_len, H, H, hd, out=ao)
-            quant_rows(ao, a8, as_)
-            gemm_fp8(a8, as_, *ly["wo"], bias=ly["bo"], residual=x, out=y)
-            layernorm_fp8(y, ly["ln1g"], ly["ln1b"], cfg.layer_norm_eps, out8=x8, scale=xs, out=x)
-            gemm_fp8(x8, xs, *ly["w1"], bias=ly["b1"], out=act, epilogue=EPI_GELU)
-            quant_rows(act, act8, acts)
-            gemm_fp8(act8, acts, *ly["w2"], bias=ly["b2"], residual=x, out=y)
-            layernorm_fp8(y, ly["ln2g"], ly["ln2b"], cfg.layer_norm_eps, out8=x8, scale=xs, out=x)
 
     @torch.no_grad()
     def embed_packed(self, batch: PackedBatch, normalize: bool = True, out_bf16: Optional[torch.Tensor] = None
                      ) -> Tuple[torch.Tensor, torch.Tensor]:
-        L = _lib.lib()
-        x = self.hidden(batch)
-        d = self.cfg.hidden_size
-        out_b = _dest(out_bf16, batch.n_seq, d, self.device)
-        out_f = torch.empty(batch.n_seq, d, dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(L.ezr_pool_normalize(_lib.ptr(x), x.stride(0), _lib.ptr(batch.cu), batch.n_seq, self.pool, 0,
-                                            None, 0.0, 2 if normalize else 0, d, _lib.ptr(out_b), _lib.ptr(out_f),
-                                            _lib.stream_ptr()), "ezr_pool_normalize")
-        return out_b, out_f
+        return _pool(self, batch, out_bf16, self.pool, None, 0.0, 2 if normalize else 0)
 
     def flops(self, lens: Sequence[int]) -> float:
         """SURVEY.md 8(d): layers*(24 L d^2 + 4 L^2 d) per sequence (ffn = 4d)."""
