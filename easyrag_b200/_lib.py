@@ -80,6 +80,7 @@ SIGNATURES = {
     "ezr_dense_s8_set_capacity": (C.c_int, [_i32]),
     "ezr_dense_set_kernel": (C.c_int, [_i32]),
     "ezr_dense_last_kernel": (C.c_char_p, []),
+    "ezr_dense_wide_workspace": (_sz, [_i64, _i32, _i32, _i32]),
     "ezr_dense_set_stage_cap": (C.c_int, [_i32]),
     "ezr_dense_set_probe": (C.c_int, [_i32]),
     "ezr_rrf_fuse": (C.c_int, [_p, _p, _p, _p, _i32, _i32, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
@@ -184,7 +185,7 @@ def require_cuda() -> None:
 PROF_SLOTS = {"bm25_cand": 8, "bm25_rescore": 9,
               "bm25_score": 0, "dense_tc": 1, "dense_simt": 2, "merge": 3, "fuse": 4,
               "enc_gemm": 5, "enc_attn": 6, "enc_other": 7,
-              "dense_s8_scan": 10, "dense_s8_rescore": 11, "dense_s8_full": 12}
+              "dense_s8_scan": 10, "dense_s8_rescore": 11, "dense_s8_full": 12, "dense_wide": 13}
 
 
 def profile_read(name: str):

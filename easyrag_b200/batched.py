@@ -44,12 +44,36 @@ class TopK:
 
 def dense_topk(index: DenseIndex, queries: torch.Tensor, k: int, q_group: Optional[torch.Tensor] = None,
                id_base: Optional[int] = None, ws: Optional[Workspace] = None, stream=None,
-               out: Optional[TopK] = None, cand_counts: Optional[torch.Tensor] = None) -> TopK:
+               out: Optional[TopK] = None, cand_counts: Optional[torch.Tensor] = None, form: Optional[int] = None,
+               block_queries: Optional[int] = None) -> TopK:
     """QdrantRetriever._aretrieve's search for a batch (retrievers.py:37-52): cosine top-k, ids descending on ties.
 
     A quantized index runs ``ezr_dense_s8_topk`` (int8 candidate pass + exact rescoring; its scores are the
     fixed-order fp32 ``rescore`` of csrc/dense_s8.cu).  ``cand_counts`` (int32 [Q] on the device, quantized indexes
-    only) receives the candidates per query of the int8 pass."""
+    only) receives the candidates per query of the int8 pass.
+
+    ``form`` forces a kernel form of ``ezr_dense_set_kernel`` for this call (the calling thread's switch is set back
+    to 0, automatic, afterwards); form 6 (wgmma score rows + select) takes any dim % 64 == 0 and k <= 1024.
+    ``block_queries`` (form 6 only) runs it in query blocks of that many queries, with a workspace of
+    ``ezr_dense_wide_workspace`` bytes; by default the block is the largest that ``ezr_dense_topk_workspace`` holds."""
+    if block_queries is not None:
+        if form != 6:
+            raise ValueError("block_queries needs form=6 (the wgmma score-row form)")
+        if getattr(index, "quantized", False):
+            raise ValueError("block_queries does not apply to a quantized index")
+        if block_queries < 1:
+            raise ValueError(f"block_queries={block_queries} must be >= 1")
+    if form is None:
+        return _dense_topk(index, queries, k, q_group, id_base, ws, stream, out, cand_counts, None, None)
+    L = _lib.lib()
+    _lib.check(L.ezr_dense_set_kernel(int(form)), "ezr_dense_set_kernel")
+    try:
+        return _dense_topk(index, queries, k, q_group, id_base, ws, stream, out, cand_counts, form, block_queries)
+    finally:
+        L.ezr_dense_set_kernel(0)
+
+
+def _dense_topk(index, queries, k, q_group, id_base, ws, stream, out, cand_counts, form, block_queries) -> TopK:
     L = _lib.lib()
     dev = index.device
     q = queries
@@ -67,9 +91,15 @@ def dense_topk(index: DenseIndex, queries: torch.Tensor, k: int, q_group: Option
     quantized = getattr(index, "quantized", False)
     if cand_counts is not None and not quantized:
         raise ValueError("cand_counts needs a quantized index")
-    need = (L.ezr_dense_s8_topk_workspace if quantized else L.ezr_dense_topk_workspace)(index.n_rows, dim, nq, k)
+    if block_queries is not None:
+        need = L.ezr_dense_wide_workspace(index.n_rows, nq, k, block_queries)
+    else:
+        need = (L.ezr_dense_s8_topk_workspace if quantized else L.ezr_dense_topk_workspace)(index.n_rows, dim, nq, k)
     ws = ws or Workspace(dev)
     buf = ws.get(need)
+    # form 6 runs the largest query block the bytes it is given hold: give it exactly the bytes sized above, so that
+    # the block does not depend on what the grow-only buffer held before
+    ws_bytes = need if form == 6 else buf.numel()
     base = index.row_lo if id_base is None else id_base
     with torch.cuda.device(dev):
         if quantized:
@@ -83,7 +113,7 @@ def dense_topk(index: DenseIndex, queries: torch.Tensor, k: int, q_group: Option
         _lib.check(L.ezr_dense_topk(_lib.ptr(index.vectors), index.n_rows, dim, index.vectors.stride(0), _lib.ptr(q), nq,
                                     q.stride(0), k, _lib.ptr(index.doc_group if qg is not None else None), _lib.ptr(qg),
                                     base, _lib.ptr(out.scores), _lib.ptr(out.ids), _lib.ptr(out.counts), _lib.ptr(buf),
-                                    buf.numel(), _lib.stream_ptr(stream)), "ezr_dense_topk")
+                                    ws_bytes, _lib.stream_ptr(stream)), "ezr_dense_topk")
     return out
 
 

@@ -6,7 +6,9 @@
 // k <= 16); everything else (odd dims, k up to 1024 as used by the drop-in
 // retrievers with f_topk_1 = 288) goes through the kernel below: a plain tiled
 // fp32-FMA score kernel writing a block of score rows, followed by the generic
-// row top-k.  Same canonical order, same filter semantics.
+// row top-k.  Same canonical order, same filter semantics.  Form 6 (dense_wide.cu,
+// opt-in through ezr_dense_set_kernel(6)) writes the score rows with wgmma instead,
+// for any dim % 64 == 0.
 #include "ezr_common.cuh"
 #include "dense_tc.h"
 #include "../../include/easyrag_b200.h"
@@ -167,9 +169,10 @@ using namespace ezr;
 extern "C" {
 
 int ezr_dense_set_kernel(int32_t which) {
-    EZR_CHECK_ARG(which >= 0 && which <= 5,
+    EZR_CHECK_ARG(which >= 0 && which <= 6,
                   "dense_set_kernel: 0 auto, 1 simt, 2 wgmma (128-query blocks, dim <= 768), 3 wgmma (64-query blocks), "
-                  "4 wgmma (64-query blocks, 128-row corpus tiles), 5 = 4 in cluster pairs (multicast corpus tiles)");
+                  "4 wgmma (64-query blocks, 128-row corpus tiles), 5 = 4 in cluster pairs (multicast corpus tiles), "
+                  "6 wgmma score rows + select (any dim %% 64 == 0, k <= 1024)");
     g_force_kernel = which;
     return EZR_OK;
 }
@@ -214,6 +217,17 @@ int ezr_dense_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t
     }
     const __nv_bfloat16* c = reinterpret_cast<const __nv_bfloat16*>(corpus_bf16);
     const __nv_bfloat16* q = reinterpret_cast<const __nv_bfloat16*>(queries_bf16);
+    if (g_force_kernel == 6) {
+        if (!dense_wide_supported(c, n_rows, dim, ld_corpus, q, ld_queries)) {
+            set_error("dense_topk: wgmma-scores kernel forced but shape unsupported (needs dim %% 64 == 0, row strides "
+                      "%% 8 == 0, 16-byte aligned rows; dim=%d ld=%lld/%lld)", dim, (long long)ld_corpus,
+                      (long long)ld_queries);
+            return EZR_ERR_UNSUPPORTED;
+        }
+        g_last_kernel = "wgmma-scores";
+        return dense_wide_topk(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k, doc_group, q_group, id_base,
+                               out_scores, out_ids, out_counts, workspace, workspace_bytes, st);
+    }
     const bool tc_ok = dense_tc_supported(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k);
     if (g_force_kernel >= 2 && !tc_ok) {
         set_error("dense_topk: wgmma kernel forced but shape unsupported (dim=%d k=%d ld=%lld)", dim, k,

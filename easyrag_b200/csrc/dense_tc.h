@@ -29,6 +29,17 @@ int dense_exact_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64
                      float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
                      cudaStream_t st);
 
+// Form 6 (dense_wide.cu): wgmma score rows for any dim % 64 == 0, then ezr_select_rows (k <= 1024).  The query block is
+// the largest whose rows and select workspace fit ws_bytes; dense_wide_workspace = the bytes for blocks of
+// block_queries queries.
+bool dense_wide_supported(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc,
+                          const __nv_bfloat16* queries, int64_t ldq);
+size_t dense_wide_workspace(int64_t n_rows, int n_queries, int k, int block_queries);
+int dense_wide_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
+                    int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
+                    float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
+                    cudaStream_t st);
+
 extern int g_dense_probe;       // see ezr_dense_set_probe
 extern int g_dense_stage_cap;   // see ezr_dense_set_stage_cap
 

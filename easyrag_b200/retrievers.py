@@ -124,10 +124,19 @@ class B200VectorStore:
     (amortised O(new nodes)); :meth:`add_embedded` takes the encoder's device tensor directly and
     :meth:`from_embed_model` lets the embedding model write its bf16 rows straight into the corpus matrix -- no
     Python float lists between the encoder and the index.
+
+    ``dense_form`` / ``block_queries`` are passed to :func:`easyrag_b200.batched.dense_topk` as ``form`` /
+    ``block_queries`` on every query (``dense_form=6``: wgmma score rows, for wide embeddings such as gte-Qwen2-7B's
+    3584 dims or k > 16); the defaults keep the automatic choice.
     """
 
-    def __init__(self, nodes: Optional[Sequence[Any]] = None, device="cuda", quantize: bool = False):
+    def __init__(self, nodes: Optional[Sequence[Any]] = None, device="cuda", quantize: bool = False,
+                 dense_form: Optional[int] = None, block_queries: Optional[int] = None):
+        if block_queries is not None and (dense_form != 6 or quantize):
+            raise ValueError("block_queries needs dense_form=6 and an index that is not quantized")
         self.device = device
+        self.dense_form = dense_form
+        self.block_queries = block_queries
         # keep an int8 mirror: exact search through a certified int8 pass (currently slower than bf16, README)
         self.quantize = bool(quantize)
         self.nodes: List[Any] = []
@@ -171,10 +180,11 @@ class B200VectorStore:
 
     @classmethod
     def from_embed_model(cls, nodes: Sequence[Any], embed_model, device="cuda", batch_size: Optional[int] = None,
-                         quantize: bool = False) -> "B200VectorStore":
+                         quantize: bool = False, dense_form: Optional[int] = None,
+                         block_queries: Optional[int] = None) -> "B200VectorStore":
         """Corpus encode written in place (replaces pipeline.py:141-158 + ingestion.py:155-191): every batch of
         ``embed_model.embed_tensor`` lands in its slice of the corpus matrix, normalised on the way."""
-        store = cls(device=device, quantize=quantize)
+        store = cls(device=device, quantize=quantize, dense_form=dense_form, block_queries=block_queries)
         nodes = list(nodes)
         bs = int(batch_size or getattr(embed_model, "embed_batch_size", 128) or 128)
         embed_type = getattr(embed_model, "_embed_type", 0)
@@ -213,7 +223,8 @@ class B200VectorStore:
         if doc_group is not None:
             self.index.doc_group = self._doc_group(tuple(conditions.keys()), doc_group)
             q_group = torch.tensor([want], dtype=torch.int32)
-        res = batched.dense_topk(self.index, q, k, q_group=q_group, ws=self._ws)
+        res = batched.dense_topk(self.index, q, k, q_group=q_group, ws=self._ws, form=self.dense_form,
+                                 block_queries=self.block_queries)
         n = int(res.counts[0])
         ids = res.ids[0, :n].tolist()
         sims = res.scores[0, :n].tolist()

@@ -209,12 +209,18 @@ int ezr_normalize_rows(const void* x, int32_t x_is_f32, int64_t ldx, int64_t n_r
 /* 0 = pick automatically, 1 = force the generic SIMT kernel, 2 = force the wgmma kernel with 128-query blocks
  * (dim <= 768; the automatic choice there), 3 = force the wgmma kernel with 64-query blocks (the automatic choice
  * above 768), 4 = 64-query blocks and 128-row corpus tiles, 5 = 4 run in cluster pairs (two neighbouring query blocks
- * on the same corpus split; each CTA loads half of every corpus tile and TMA-multicasts it to both); 2-5 error if the
- * shape is unsupported */
+ * on the same corpus split; each CTA loads half of every corpus tile and TMA-multicasts it to both), 6 = wgmma score
+ * rows of a query block, then the generic row top-k (any dim % 64 == 0, any k <= 1024; never chosen automatically);
+ * 2-6 error if the shape is unsupported */
 int ezr_dense_set_kernel(int32_t which);
 /* name of the kernel the last ezr_dense_topk call on this thread launched
- * ("wgmma" / "wgmma-q64" / "wgmma-q64-n128" / "wgmma-q64-n128-mc2" / "simt") */
+ * ("wgmma" / "wgmma-q64" / "wgmma-q64-n128" / "wgmma-q64-n128-mc2" / "wgmma-scores" / "simt") */
 const char* ezr_dense_last_kernel(void);
+/* Workspace of form 6 run in query blocks of block_queries queries: their fp32 score rows plus the select workspace
+ * (of the smaller last block too).  Form 6 runs the largest block whose bytes fit the workspace it is given, so this
+ * many bytes run blocks of block_queries queries; ezr_dense_topk_workspace's bytes run blocks at least as large as
+ * the SIMT kernel's (256 MB of score rows).  Fewer bytes than block_queries = 1 needs: EZR_ERR_WORKSPACE. */
+size_t ezr_dense_wide_workspace(int64_t n_rows, int32_t n_queries, int32_t k, int32_t block_queries);
 
 /* Cap the TMA ring of the wgmma kernel at `stages` stages (0 = use all shared memory, the default).  A capped
  * ring leaves shared memory on an SM for kernels of another stream only when the resident query block is small; a
@@ -440,7 +446,8 @@ typedef enum ezr_prof_slot {
     EZR_PROF_DENSE_S8_SCAN = 10,    /* dense_s8_prep_kernel + dense_s8_scan_kernel (int8 candidate pass) */
     EZR_PROF_DENSE_S8_RESCORE = 11, /* dense_s8_rescore_kernel (exact rescoring + top-k of the candidates) */
     EZR_PROF_DENSE_S8_FULL = 12,    /* full scan of overflowed queries / k > 16 (gather + score rows + select) */
-    EZR_PROF_COUNT = 13
+    EZR_PROF_DENSE_WIDE = 13,       /* dense_scores_wgmma_kernel (form 6 score rows; the select counts as merge) */
+    EZR_PROF_COUNT = 14
 } ezr_prof_slot;
 /* kernels launched by this library since it was loaded (every launch site counts itself) */
 long long ezr_launch_count(void);
