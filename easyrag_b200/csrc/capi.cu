@@ -1,5 +1,6 @@
-// Library-wide C ABI plumbing: version, thread-local error text, device check.
+// Library-wide C ABI plumbing: version, thread-local error text, device check; host helpers every kernel file uses.
 #include "ezr_common.cuh"
+#include "ptx.cuh"
 #include "../../include/easyrag_b200.h"
 #include <stdarg.h>
 #include <utility>
@@ -26,6 +27,42 @@ int sm_count() {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
     cached = n;
     return n;
+}
+
+// ---------------------------------------------------------- tensor maps ----
+// encode_tmap_2d_bf16 (declared in ptx.cuh): the GEMMs, attention, the dense forms and the int8 scan all use it.
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+int encode_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_elems,
+                        uint32_t box_cols, uint32_t box_rows, int swizzle_bytes) {
+    static PFN_encodeTiled fn = nullptr;
+    if (!fn) {
+        void* sym = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        EZR_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres));
+        if (qres != cudaDriverEntryPointSuccess || !sym) {
+            set_error("cuTensorMapEncodeTiled not available from the driver");
+            return EZR_ERR_CUDA;
+        }
+        fn = reinterpret_cast<PFN_encodeTiled>(sym);
+    }
+    cuuint64_t gdim[2] = {cols, rows};
+    cuuint64_t gstride[1] = {row_stride_elems * 2};
+    cuuint32_t box[2] = {box_cols, box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE,
+                    swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled failed (%d): cols=%llu rows=%llu stride=%llu box=%ux%u", (int)r,
+                  (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)row_stride_elems, box_cols,
+                  box_rows);
+        return EZR_ERR_CUDA;
+    }
+    return EZR_OK;
 }
 
 // ------------------------------------------------------------- profiler ----

@@ -7,8 +7,8 @@
 // retrievers with f_topk_1 = 288) goes through the kernel below: a plain tiled
 // fp32-FMA score kernel writing a block of score rows, followed by the generic
 // row top-k.  Same canonical order, same filter semantics.  Form 6 (dense_wide.cu,
-// opt-in through ezr_dense_set_kernel(6)) writes the score rows with wgmma instead,
-// for any dim % 64 == 0.
+// opt-in through ezr_dense_set_kernel(6)) writes the score rows with the encoder's
+// wgmma GEMM instead, for any dim % 64 == 0; both go through score_rows_topk below.
 #include "ezr_common.cuh"
 #include "dense_tc.h"
 #include "../../include/easyrag_b200.h"
@@ -81,37 +81,55 @@ static int simt_block_queries(int64_t n_rows, int n_queries) {
     return (int)qb;
 }
 
-static size_t simt_workspace(int64_t n_rows, int n_queries, int k) {
-    const int qb = simt_block_queries(n_rows, n_queries);
-    return align_up((size_t)qb * n_rows * 4, 256) + ezr_select_rows_workspace(qb, n_rows, k, EZR_F32);
+template <bool SEP>
+static int simt_scores(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc,
+                       const __nv_bfloat16* queries, int nq, int64_t ldq, float* out, cudaStream_t st) {
+    dim3 grid(ceil_div(n_rows, kSimtTile), ceil_div(nq, kSimtTile));
+    {
+        ProfScope prof(EZR_PROF_DENSE_SIMT, st);
+        dense_scores_simt_kernel<SEP><<<grid, 256, 0, st>>>(corpus, n_rows, dim, ldc, queries, nq, ldq, out, n_rows);
+    }
+    EZR_LAUNCH_CHECK();
+    return EZR_OK;
 }
 
-template <bool SEP>
-static int simt_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64_t ldc, const __nv_bfloat16* queries,
-                     int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
-                     float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
-                     cudaStream_t st) {
-    const size_t need = simt_workspace(n_rows, n_queries, k);
+// A block of m queries: its score rows, then the select workspace behind them.  The last block of a call may be
+// smaller than the others and its select may need more (it splits each row into more parts); its rows take less room.
+static size_t score_block_bytes(int64_t n_rows, int m, int k) {
+    return align_up((size_t)m * n_rows * 4, 256) + ezr_select_rows_workspace(m, n_rows, k, EZR_F32);
+}
+
+size_t score_rows_workspace(int64_t n_rows, int n_queries, int k, int block_queries) {
+    if (n_rows <= 0 || n_queries <= 0 || k <= 0 || block_queries <= 0) return 0;
+    const int qb = block_queries < n_queries ? block_queries : n_queries;
+    size_t need = score_block_bytes(n_rows, qb, k);
+    const int last = n_queries % qb;
+    if (last) {
+        const size_t l = score_block_bytes(n_rows, last, k);
+        if (l > need) need = l;
+    }
+    return need;
+}
+
+int score_rows_topk(score_rows_fn score, int block_queries, const __nv_bfloat16* corpus, int64_t n_rows, int dim,
+                    int64_t ldc, const __nv_bfloat16* queries, int n_queries, int64_t ldq, int k,
+                    const int32_t* doc_group, const int32_t* q_group, int id_base, float* out_scores, int32_t* out_ids,
+                    int32_t* out_counts, void* ws, size_t ws_bytes, cudaStream_t st) {
+    const size_t need = score_rows_workspace(n_rows, n_queries, k, block_queries);
     if (ws_bytes < need || !ws) {
-        set_error("dense_topk(simt): workspace %zu < %zu", ws_bytes, need);
+        set_error("dense_topk: workspace %zu < %zu (score rows of %d-query blocks)", ws_bytes, need, block_queries);
         return EZR_ERR_WORKSPACE;
     }
-    const int qb = simt_block_queries(n_rows, n_queries);
     float* rows = reinterpret_cast<float*>(ws);
-    const size_t rows_bytes = align_up((size_t)qb * n_rows * 4, 256);
-    void* sel_ws = (char*)ws + rows_bytes;
-    for (int q0 = 0; q0 < n_queries; q0 += qb) {
-        const int nq = n_queries - q0 < qb ? n_queries - q0 : qb;
-        dim3 grid(ceil_div(n_rows, kSimtTile), ceil_div(nq, kSimtTile));
-        {
-            ProfScope prof(EZR_PROF_DENSE_SIMT, st);
-            dense_scores_simt_kernel<SEP><<<grid, 256, 0, st>>>(corpus, n_rows, dim, ldc, queries + (int64_t)q0 * ldq, nq,
-                                                           ldq, rows, n_rows);
-        }
-        EZR_LAUNCH_CHECK();
-        int rc = ezr_select_rows(rows, EZR_F32, nq, n_rows, n_rows, k, 0, doc_group, q_group ? q_group + q0 : nullptr,
-                                 id_base, out_scores + (int64_t)q0 * k, out_ids + (int64_t)q0 * k,
-                                 out_counts ? out_counts + q0 : nullptr, sel_ws, ws_bytes - rows_bytes, st);
+    for (int q0 = 0; q0 < n_queries; q0 += block_queries) {
+        const int nq = n_queries - q0 < block_queries ? n_queries - q0 : block_queries;
+        int rc = score(corpus, n_rows, dim, ldc, queries + (int64_t)q0 * ldq, nq, ldq, rows, st);
+        if (rc) return rc;
+        // this block's select workspace sits right behind its own rows (see score_block_bytes)
+        const size_t rows_bytes = align_up((size_t)nq * n_rows * 4, 256);
+        rc = ezr_select_rows(rows, EZR_F32, nq, n_rows, n_rows, k, 0, doc_group, q_group ? q_group + q0 : nullptr,
+                             id_base, out_scores + (int64_t)q0 * k, out_ids + (int64_t)q0 * k,
+                             out_counts ? out_counts + q0 : nullptr, (char*)ws + rows_bytes, ws_bytes - rows_bytes, st);
         if (rc) return rc;
     }
     return EZR_OK;
@@ -133,8 +151,9 @@ int dense_exact_topk(const __nv_bfloat16* corpus, int64_t n_rows, int dim, int64
                      int n_queries, int64_t ldq, int k, const int32_t* doc_group, const int32_t* q_group, int id_base,
                      float* out_scores, int32_t* out_ids, int32_t* out_counts, void* ws, size_t ws_bytes,
                      cudaStream_t st) {
-    return simt_topk<true>(corpus, n_rows, dim, ldc, queries, n_queries, ldq, k, doc_group, q_group, id_base,
-                           out_scores, out_ids, out_counts, ws, ws_bytes, st);
+    return score_rows_topk(simt_scores<true>, simt_block_queries(n_rows, n_queries), corpus, n_rows, dim, ldc, queries,
+                           n_queries, ldq, k, doc_group, q_group, id_base, out_scores, out_ids, out_counts, ws, ws_bytes,
+                           st);
 }
 
 static thread_local int g_force_kernel = 0;
@@ -193,7 +212,7 @@ int ezr_dense_set_stage_cap(int32_t stages) {
 
 size_t ezr_dense_topk_workspace(int64_t n_rows, int32_t dim, int32_t n_queries, int32_t k) {
     if (n_rows <= 0 || n_queries <= 0 || k <= 0) return 0;
-    size_t a = simt_workspace(n_rows, n_queries, k);
+    size_t a = score_rows_workspace(n_rows, n_queries, k, simt_block_queries(n_rows, n_queries));
     size_t b = dense_tc_workspace(n_rows, dim, n_queries, k);
     return a > b ? a : b;
 }
@@ -246,8 +265,9 @@ int ezr_dense_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t
                              out_scores, out_ids, out_counts, workspace, workspace_bytes, st, form);
     }
     g_last_kernel = "simt";
-    return simt_topk<false>(c, n_rows, dim, ld_corpus, q, n_queries, ld_queries, k, doc_group, q_group, id_base, out_scores,
-                     out_ids, out_counts, workspace, workspace_bytes, st);
+    return score_rows_topk(simt_scores<false>, simt_block_queries(n_rows, n_queries), c, n_rows, dim, ld_corpus, q,
+                           n_queries, ld_queries, k, doc_group, q_group, id_base, out_scores, out_ids, out_counts,
+                           workspace, workspace_bytes, st);
 }
 
 int ezr_normalize_rows(const void* x, int32_t x_is_f32, int64_t ldx, int64_t n_rows, int32_t dim, void* out_bf16,

@@ -502,40 +502,6 @@ dense_wgmma_rq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
 }
 
 // ------------------------------------------------------------------ host ----
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int encode_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_elems,
-                        uint32_t box_cols, uint32_t box_rows, int swizzle_bytes) {
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* sym = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        EZR_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres));
-        if (qres != cudaDriverEntryPointSuccess || !sym) {
-            set_error("cuTensorMapEncodeTiled not available from the driver");
-            return EZR_ERR_CUDA;
-        }
-        fn = reinterpret_cast<PFN_encodeTiled>(sym);
-    }
-    cuuint64_t gdim[2] = {cols, rows};
-    cuuint64_t gstride[1] = {row_stride_elems * 2};
-    cuuint32_t box[2] = {box_cols, box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled failed (%d): cols=%llu rows=%llu stride=%llu box=%ux%u", (int)r,
-                  (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)row_stride_elems, box_cols,
-                  box_rows);
-        return EZR_ERR_CUDA;
-    }
-    return EZR_OK;
-}
-
 int tc_rows_per_slice(int64_t n_rows, int slices, int tn) {
     const int64_t tiles = (n_rows + tn - 1) / tn;
     return (int)((tiles + slices - 1) / slices) * tn;

@@ -1,13 +1,14 @@
 // Epilogue shared by the encoder GEMMs (gemm_tc.cu: bf16 wgmma, gemm_fp8.cu: e4m3 wgmma).  Both kernels hand it one
 // pair of adjacent output columns of one row, in fp32, after their own accumulation; it adds the bias, applies GELU or
-// SwiGLU, adds the residual and stores bf16.
+// SwiGLU, adds the residual and stores bf16.  EPI_SCORES (gemm_tc.cu only) stores the fp32 dot products themselves:
+// the score rows of dense top-k form 6 (dense_wide.cu).
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
 
 namespace ezr {
 
-enum { EPI_NONE = 0, EPI_GELU = 1, EPI_SWIGLU = 2 };
+enum { EPI_NONE = 0, EPI_GELU = 1, EPI_SWIGLU = 2, EPI_SCORES = 3 };
 
 // erf GELU (HF "gelu"): gelu(x) = 0.5 x (1 + erf(x / sqrt 2)).  erfc(|z|) = t (a1 + t (a2 + t (a3 + t (a4 + t a5)))) exp(-z^2),
 // t = 1 / (1 + p |z|) (Abramowitz & Stegun 7.1.26, |error| <= 1.5e-7), evaluated through erfc on BOTH sides so the
@@ -37,14 +38,26 @@ __device__ __forceinline__ void store_pair(__nv_bfloat16* o, bool pair_ok, bool 
         if (second) o[1] = __float2bfloat16(x1);
     }
 }
+__device__ __forceinline__ void store_pair(float* o, bool pair_ok, bool second, float x0, float x1) {
+    if (pair_ok && second) {
+        *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
+    } else {
+        o[0] = x0;
+        if (second) o[1] = x1;
+    }
+}
 
 // One pair of outputs: x0 / x1 are accumulator columns col, col + 1 (the gate columns for SwiGLU, whose "up" columns
 // col + UP, col + UP + 1 arrive as u0 / u1; UP is half the kernel's tile width).  ocol is the output column, `second`
-// says whether ocol + 1 is inside the output, rrow is the residual row or null.
-template <int EPI, int UP>
+// says whether ocol + 1 is inside the output, rrow is the residual row or null.  OUT: __nv_bfloat16, float for EPI_SCORES.
+template <int EPI, int UP, typename OUT>
 __device__ __forceinline__ void epilogue_pair(float x0, float x1, float u0, float u1, const __nv_bfloat16* bias, int col,
-                                              const __nv_bfloat16* rrow, bool res_pair, __nv_bfloat16* orow,
+                                              const __nv_bfloat16* rrow, bool res_pair, OUT* orow,
                                               bool out_pair, int ocol, bool second) {
+    if constexpr (EPI == EPI_SCORES) {         // no bias, no residual; -0.0 -> +0.0 as in every dense form
+        store_pair(orow + ocol, out_pair, second, x0 + 0.0f, x1 + 0.0f);
+        return;
+    }
     if (EPI == EPI_SWIGLU) {
         if (bias) {
             x0 += __bfloat162float(bias[col]);

@@ -17,8 +17,15 @@
 // Tile order: N tiles fastest.  The activations of a 147k-token batch (226 MB at K = 768, 905 MB at K = 3072) do not fit
 // the 50 MB L2, the weights (a few MB) do: with N fastest the CTAs in flight cover a few M tiles x all N tiles, so an A
 // tile is fetched from HBM about once.
+//
+// Dense top-k form 6 (dense_wide.cu) runs the same kernel on A = a block of queries, W = the corpus rows, with the
+// EPI_SCORES epilogue (fp32 score rows, gemm_scores_f32) and M tiles fastest: there the query block (a few MB) fits L2
+// and the corpus does not, so the CTAs in flight cover all query tiles of a few corpus tiles.
+#include <type_traits>
+
 #include "../ezr_common.cuh"
 #include "../ptx.cuh"
+#include "../dense_tc.h"
 #include "gemm_epi.cuh"
 
 namespace ezr {
@@ -35,7 +42,7 @@ struct GemmParams {
     const __nv_bfloat16* bias;       // [N] or null
     const __nv_bfloat16* residual;   // [M, ldr] or null
     int64_t ldr;
-    __nv_bfloat16* out;              // [M, ldo]
+    void* out;                       // [M, ldo] bf16; fp32 for EPI_SCORES
     int64_t ldo;
 };
 
@@ -44,7 +51,7 @@ struct GemmBarriers {
     uint64_t empty[G_STAGES];
 };
 
-template <int EPI>
+template <int EPI, bool M_FAST>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const GemmParams p) {
     extern __shared__ __align__(1024) unsigned char smem_dyn[];
@@ -52,7 +59,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     unsigned char* smem_a = smem;
     unsigned char* smem_b = smem + (size_t)G_STAGES * G_A_BYTES;
     GemmBarriers* bars = reinterpret_cast<GemmBarriers*>(smem_b + (size_t)G_STAGES * G_B_BYTES);
-    const int tn = blockIdx.x % p.tiles_n, tm = blockIdx.x / p.tiles_n;     // N tiles fastest: see the header
+    // N tiles fastest, M tiles for the score rows: see the header
+    const int tn = M_FAST ? blockIdx.x / p.tiles_m : blockIdx.x % p.tiles_n;
+    const int tm = M_FAST ? blockIdx.x % p.tiles_m : blockIdx.x / p.tiles_n;
     const int kchunks = p.K / GK;
     const int wg = threadIdx.x >> 7;
 
@@ -104,8 +113,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     // (the last stage is never handed back: no later load of this CTA needs it)
 
     // ---------------- epilogue on the accumulator registers
+    typedef typename std::conditional<EPI == EPI_SCORES, float, __nv_bfloat16>::type out_t;
     const int n_out = (EPI == EPI_SWIGLU) ? p.N / 2 : p.N;
-    const bool out_pair = (p.ldo % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 3) == 0);
+    const bool out_pair = (p.ldo % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & (2 * sizeof(out_t) - 1)) == 0);
     const bool res_pair = p.residual && (p.ldr % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0);
     const int cq = (lane & 3) * 2;
     constexpr int NJ = (EPI == EPI_SWIGLU) ? GN / 16 : GN / 8;       // 8-column groups of output per thread row
@@ -113,7 +123,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     for (int h = 0; h < 2; ++h) {
         const int row = tm * GM + cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
         if (row >= p.M) continue;
-        __nv_bfloat16* orow = p.out + (int64_t)row * p.ldo;
+        out_t* orow = static_cast<out_t*>(p.out) + (int64_t)row * p.ldo;
         const __nv_bfloat16* rrow = p.residual ? p.residual + (int64_t)row * p.ldr : nullptr;
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
@@ -130,12 +140,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 }
 
 static int gemm_launch(const __nv_bfloat16* A, int M, int K, int64_t lda, const __nv_bfloat16* W, int N, int64_t ldw,
-                       const __nv_bfloat16* bias, const __nv_bfloat16* residual, int64_t ldr, __nv_bfloat16* out,
-                       int64_t ldo, int epi, cudaStream_t st) {
+                       const __nv_bfloat16* bias, const __nv_bfloat16* residual, int64_t ldr, void* out,
+                       int64_t ldo, int epi, int prof_slot, cudaStream_t st) {
     EZR_CHECK_ARG(M >= 0 && N >= 1 && K >= GK && K % GK == 0, "gemm: need K %% 64 == 0 (M=%d N=%d K=%d)", M, N, K);
     EZR_CHECK_ARG(lda % 8 == 0 && ldw % 8 == 0 && lda >= K && ldw >= K, "gemm: row strides must be multiples of 8 and >= K");
     EZR_CHECK_ARG(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W)) & 15) == 0, "gemm: A/W must be 16-byte aligned");
-    EZR_CHECK_ARG(epi >= EPI_NONE && epi <= EPI_SWIGLU, "gemm: bad epilogue %d", epi);
     EZR_CHECK_ARG(epi != EPI_SWIGLU || N % GN == 0, "gemm: SwiGLU epilogue needs N %% 256 == 0 (gate/up interleaved in blocks of 128 rows)");
     if (M == 0) return EZR_OK;
     GemmParams p;
@@ -150,8 +159,9 @@ static int gemm_launch(const __nv_bfloat16* A, int M, int K, int64_t lda, const 
     if (rc) return rc;
     const size_t smem = 1024 + (size_t)G_STAGES * (G_A_BYTES + G_B_BYTES) + sizeof(GemmBarriers);
     typedef void (*kern_t)(const CUtensorMap, const CUtensorMap, const GemmParams);
-    static const kern_t table[3] = {gemm_wgmma_kernel<EPI_NONE>, gemm_wgmma_kernel<EPI_GELU>, gemm_wgmma_kernel<EPI_SWIGLU>};
-    static bool attr_done[3] = {false, false, false};
+    static const kern_t table[4] = {gemm_wgmma_kernel<EPI_NONE, false>, gemm_wgmma_kernel<EPI_GELU, false>,
+                                    gemm_wgmma_kernel<EPI_SWIGLU, false>, gemm_wgmma_kernel<EPI_SCORES, true>};
+    static bool attr_done[4] = {false, false, false, false};
     if (!attr_done[epi]) {
         EZR_CUDA(cudaFuncSetAttribute(table[epi], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done[epi] = true;
@@ -159,11 +169,16 @@ static int gemm_launch(const __nv_bfloat16* A, int M, int K, int64_t lda, const 
     const long long tiles = (long long)p.tiles_m * p.tiles_n;
     EZR_CHECK_ARG(tiles < (1ll << 31), "gemm: too many tiles");
     {
-        ProfScope prof(EZR_PROF_ENC_GEMM, st);
+        ProfScope prof(prof_slot, st);
         table[epi]<<<(unsigned)tiles, G_THREADS, smem, st>>>(map_a, map_w, p);
     }
     EZR_LAUNCH_CHECK();
     return EZR_OK;
+}
+
+int gemm_scores_f32(const __nv_bfloat16* A, int M, int K, int64_t lda, const __nv_bfloat16* W, int N, int64_t ldw,
+                    float* out, int64_t ldo, int prof_slot, cudaStream_t st) {
+    return gemm_launch(A, M, K, lda, W, N, ldw, nullptr, nullptr, 0, out, ldo, EPI_SCORES, prof_slot, st);
 }
 
 }  // namespace ezr
@@ -172,6 +187,7 @@ extern "C" int ezr_gemm_bf16(const void* a, int32_t m, int32_t k, int64_t lda, c
                              const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo,
                              int32_t epilogue, void* stream) {
     using namespace ezr;
+    EZR_CHECK_ARG(epilogue >= EPI_NONE && epilogue <= EPI_SWIGLU, "gemm: bad epilogue %d", epilogue);
     return gemm_launch((const __nv_bfloat16*)a, m, k, lda, (const __nv_bfloat16*)w, n, ldw, (const __nv_bfloat16*)bias,
-                       (const __nv_bfloat16*)residual, ldr, (__nv_bfloat16*)out, ldo, epilogue, (cudaStream_t)stream);
+                       (const __nv_bfloat16*)residual, ldr, out, ldo, epilogue, EZR_PROF_ENC_GEMM, (cudaStream_t)stream);
 }

@@ -438,7 +438,7 @@ typedef enum ezr_prof_slot {
     EZR_PROF_DENSE_SIMT = 2, /* dense_scores_simt_kernel */
     EZR_PROF_MERGE = 3,      /* merge / select kernels */
     EZR_PROF_FUSE = 4,       /* rrf / simple fusion */
-    EZR_PROF_ENC_GEMM = 5,   /* encoder GEMMs */
+    EZR_PROF_ENC_GEMM = 5,   /* encoder GEMMs (not form 6's score rows: EZR_PROF_DENSE_WIDE) */
     EZR_PROF_ENC_ATTN = 6,   /* encoder attention */
     EZR_PROF_ENC_OTHER = 7,  /* encoder norms / elementwise */
     EZR_PROF_BM25_CAND = 8,  /* bm25_cand_kernel (integer candidate pass over packed postings) */
@@ -446,7 +446,7 @@ typedef enum ezr_prof_slot {
     EZR_PROF_DENSE_S8_SCAN = 10,    /* dense_s8_prep_kernel + dense_s8_scan_kernel (int8 candidate pass) */
     EZR_PROF_DENSE_S8_RESCORE = 11, /* dense_s8_rescore_kernel (exact rescoring + top-k of the candidates) */
     EZR_PROF_DENSE_S8_FULL = 12,    /* full scan of overflowed queries / k > 16 (gather + score rows + select) */
-    EZR_PROF_DENSE_WIDE = 13,       /* dense_scores_wgmma_kernel (form 6 score rows; the select counts as merge) */
+    EZR_PROF_DENSE_WIDE = 13,       /* gemm_wgmma_kernel's score-row instance (form 6; the select counts as merge) */
     EZR_PROF_COUNT = 14
 } ezr_prof_slot;
 /* kernels launched by this library since it was loaded (every launch site counts itself) */

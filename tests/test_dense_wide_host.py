@@ -39,6 +39,21 @@ def test_default_workspace_holds_the_simt_block(lib_built):
     assert L.ezr_dense_topk_workspace(n, 3584, nq, k) >= L.ezr_dense_wide_workspace(n, nq, k, 671)
 
 
+@pytest.mark.parametrize("n,nq,k", [(100_000, 700, 288), (1_000_000, 100, 288), (129, 1025, 1024), (5000, 1500, 10),
+                                    (100_000, 671, 288)])
+def test_default_workspace_covers_every_simt_block(lib_built, n, nq, k):
+    # form 1 / the SIMT fallback runs blocks of up to 1024 queries and 256 MB of score rows; each block's select
+    # workspace follows its own rows, so a smaller last block counts on its own (no wgmma form at dim 3584)
+    L = _lib.lib()
+
+    def block(m):
+        return _align(m * n * 4) + L.ezr_select_rows_workspace(m, n, k, _lib.F32)
+
+    qb = min(nq, 1024, max(1, (256 << 20) // (n * 4)))
+    want = block(qb) if nq % qb == 0 else max(block(qb), block(nq % qb))
+    assert L.ezr_dense_topk_workspace(n, 3584, nq, k) == want
+
+
 def test_block_queries_refusals():
     class _Index:
         quantized = True

@@ -54,8 +54,8 @@ def _run(form, index, q, k, q_group=None, **kw):
     return res
 
 
-def _raw(c, q, k, doc_group=None, q_group=None, id_base=0, ws_bytes=None):
-    """ezr_dense_topk under form 6 on any (possibly strided) views, with exactly ``ws_bytes`` of workspace (default:
+def _raw(c, q, k, doc_group=None, q_group=None, id_base=0, ws_bytes=None, form=6):
+    """ezr_dense_topk under ``form`` on any (possibly strided) views, with exactly ``ws_bytes`` of workspace (default:
     ezr_dense_topk_workspace).  -> (status, TopK)."""
     L = _lib.lib()
     n, d = c.shape
@@ -65,14 +65,14 @@ def _raw(c, q, k, doc_group=None, q_group=None, id_base=0, ws_bytes=None):
     if ws_bytes is None:
         ws_bytes = L.ezr_dense_topk_workspace(n, d, nq, k)
     buf = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=DEV)
-    _lib.check(L.ezr_dense_set_kernel(6))
+    _lib.check(L.ezr_dense_set_kernel(form))
     try:
         rc = L.ezr_dense_topk(_lib.ptr(c), n, d, c.stride(0), _lib.ptr(q), nq, q.stride(0), k, _lib.ptr(doc_group),
                               _lib.ptr(q_group), id_base, _lib.ptr(out.scores), _lib.ptr(out.ids), _lib.ptr(out.counts),
                               _lib.ptr(buf), ws_bytes, _lib.stream_ptr())
         torch.cuda.synchronize()
         if rc == 0 and n > 0:
-            assert L.ezr_dense_last_kernel() == b"wgmma-scores"
+            assert L.ezr_dense_last_kernel() == FORM_NAMES[form]
     finally:
         L.ezr_dense_set_kernel(0)
     return rc, out
@@ -153,6 +153,18 @@ def test_block_size_does_not_change_results(int_case):
     rc, _ = _raw(c, q[:65], k, ws_bytes=one - 1)
     assert rc == EZR_ERR_WORKSPACE
     assert b"workspace" in L.ezr_last_error()
+
+
+def test_simt_blocks_fit_the_default_workspace(int_case):
+    # form 1 runs SIMT blocks of 671 + 29 queries here.  The 29-query block's select splits each row into more parts
+    # and needs more workspace than the 671-query block's; it sits right behind the block's own rows, so exactly
+    # ezr_dense_topk_workspace holds it.
+    c, q, k = int_case["c"], int_case["q"], 288
+    rc, simt = _raw(c, q, k, form=1)
+    assert rc == 0
+    rc, wide = _raw(c, q, k)
+    assert rc == 0
+    _assert_same(simt, wide)
 
 
 def test_block_queries_needs_form_6(int_case):
