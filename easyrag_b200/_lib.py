@@ -185,7 +185,8 @@ def require_cuda() -> None:
 PROF_SLOTS = {"bm25_cand": 8, "bm25_rescore": 9,
               "bm25_score": 0, "dense_tc": 1, "dense_simt": 2, "merge": 3, "fuse": 4,
               "enc_gemm": 5, "enc_attn": 6, "enc_other": 7,
-              "dense_s8_scan": 10, "dense_s8_rescore": 11, "dense_s8_full": 12, "dense_wide": 13}
+              "dense_s8_scan": 10, "dense_s8_rescore": 11, "dense_s8_full": 12, "dense_wide": 13,
+              "bm25_bound": 14}
 
 
 def profile_read(name: str):

@@ -636,14 +636,22 @@ static bool pk_usable(const ezr_bm25_index* ix, int k) {
     return kPkEnabled && ix->post_pk != nullptr && ix->monotone && ix->score_type == EZR_F64 && k <= 32;
 }
 
+// the deep form of the two-phase path (bm25_pk.cuh): the same index types, 32 < k <= kSelMaxK
+static bool pk_deep_usable(const ezr_bm25_index* ix, int k) {
+    return kPkEnabled && ix->post_pk != nullptr && ix->monotone && ix->score_type == EZR_F64 && k > 32 &&
+           k <= kSelMaxK;
+}
+
 struct PkWorkspace {
     int32_t *thr_key, *thr_q, *cand_cnt, *ovf, *ne_sum, *ovf_n, *ovf_list, *cand_ids, *cand_q, *cand_u;
     uint32_t* ne_mask;
     int2* plan;
+    double* rows;   // deep form: [Q][list_cap] exact scores beside cand_ids
     size_t zero_bytes, total;
 };
 
-static PkWorkspace pk_carve(void* base, int n_queries) {
+// list_cap: candidates per query (kPkListCap, or pk_deep_list_cap(k) with deep, which adds the score rows)
+static PkWorkspace pk_carve(void* base, int n_queries, int list_cap = kPkListCap, bool deep = false) {
     PkWorkspace w;
     const size_t q = (size_t)n_queries;
     char* b = reinterpret_cast<char*>(base);
@@ -658,21 +666,25 @@ static PkWorkspace pk_carve(void* base, int n_queries) {
     size_t off = align_up(w.zero_bytes, 256);
     w.ovf_list = reinterpret_cast<int32_t*>(b + off);
     off += align_up(q * 4, 256);
+    const size_t lc = (size_t)list_cap;
     w.cand_ids = reinterpret_cast<int32_t*>(b + off);
-    off += align_up(q * kPkListCap * 4, 256);
+    off += align_up(q * lc * 4, 256);
     w.cand_q = reinterpret_cast<int32_t*>(b + off);
-    off += align_up(q * kPkListCap * 4, 256);
+    off += align_up(q * lc * 4, 256);
     w.cand_u = reinterpret_cast<int32_t*>(b + off);
-    off += align_up(q * kPkListCap * 4, 256);
+    off += align_up(q * lc * 4, 256);
     w.plan = reinterpret_cast<int2*>(b + off);
     off += align_up(q * kPkMaxChunk * kPkPlanTok * sizeof(int2), 256);
+    w.rows = deep ? reinterpret_cast<double*>(b + off) : nullptr;
+    if (deep) off += align_up(q * lc * 8, 256);
     w.total = off;
     return w;
 }
 
+// deep: the deep form's kernels; rescoring then fills w.rows instead of the outputs (the caller selects the top-k)
 static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t* q_terms, int n_queries, int k,
                      const int32_t* q_group, int id_base, const PkWorkspace& w, double* out_scores,
-                     int32_t* out_ids, int32_t* out_counts, cudaStream_t st) {
+                     int32_t* out_ids, int32_t* out_counts, cudaStream_t st, bool deep = false) {
     Bm25Params p;
     p.indptr = ix->indptr; p.post_doc = ix->post_doc; p.post_w = ix->post_w; p.range_off = ix->range_off;
     p.doc_group = ix->doc_group; p.q_ptr = q_ptr; p.q_terms = q_terms; p.q_group = q_group;
@@ -683,13 +695,23 @@ static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32
     c.post_pk = ix->post_pk; c.thr_q = w.thr_q; c.cand_cnt = w.cand_cnt; c.cand_ids = w.cand_ids; c.cand_q = w.cand_q; c.cand_u = w.cand_u; c.ovf = w.ovf;
     c.term_max = g_bm25_skip ? ix->term_max : nullptr; c.ne_mask = w.ne_mask; c.ne_sum = w.ne_sum;
     c.ovf_n = w.ovf_n; c.ovf_list = w.ovf_list; c.plan = g_bm25_plan ? w.plan : nullptr;
-    const size_t smem = (size_t)(kBmRange + 32) * 4;
-    static bool attr_done = false;
-    if (!attr_done) {
-        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+    const size_t smem = deep ? pk_deep_cand_smem(k) : (size_t)(kBmRange + 32) * 4;
+    const size_t bd_smem = deep ? pk_deep_bound_smem(k) : 0;
+    static bool attr_done = false, deep_attr_done = false;
+    if (!deep && !attr_done) {
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                       cudaSharedmemCarveoutMaxShared));
         attr_done = true;
+    }
+    if (deep && !deep_attr_done) {                      // sized for the largest k
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)pk_deep_cand_smem(kSelMaxK)));
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                      cudaSharedmemCarveoutMaxShared));
+        EZR_CUDA(cudaFuncSetAttribute(bm25_bound_deep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)pk_deep_bound_smem(kSelMaxK)));
+        deep_attr_done = true;
     }
     // Document ranges go in chunks of doubling size (4, 4, 8, 16, ...); between chunks every query's bound is
     // raised to the k-th best of all candidates so far, so the expected number of candidates a chunk adds stays
@@ -707,11 +729,14 @@ static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32
                 bm25_plan_kernel<<<(unsigned)((n_plan + 255) / 256), 256, 0, st>>>(p, r0, len, n_queries, w.plan);
                 EZR_LAUNCH_CHECK();
             }
-            bm25_cand_kernel<<<dim3(n_queries, len), kPkThreads, smem, st>>>(p, c, r0);
+            if (deep) bm25_cand_kernel<true><<<dim3(n_queries, len), kPkThreads, smem, st>>>(p, c, r0);
+            else bm25_cand_kernel<false><<<dim3(n_queries, len), kPkThreads, smem, st>>>(p, c, r0);
             EZR_LAUNCH_CHECK();
             r0 += len;
             if (r0 < ix->n_ranges) {
-                bm25_bound_kernel<<<n_queries, kBdThreads, 0, st>>>(p, c);
+                ProfScope prof_bd(EZR_PROF_BM25_BOUND, st);   // inside the candidate span
+                if (deep) bm25_bound_deep_kernel<<<n_queries, kBdThreads, bd_smem, st>>>(p, c);
+                else bm25_bound_kernel<<<n_queries, kBdThreads, 0, st>>>(p, c);
                 EZR_LAUNCH_CHECK();
             }
             if (r0 > first && span < kPkMaxChunk) span *= 2;
@@ -719,7 +744,8 @@ static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32
     }
     {
         ProfScope prof(EZR_PROF_BM25_RESCORE, st);
-        bm25_rescore_kernel<<<n_queries, kRsThreads, 0, st>>>(p, c, out_scores, out_ids, out_counts);
+        if (deep) bm25_rescore_deep_kernel<<<n_queries, kRsThreads, 0, st>>>(p, c, w.rows);
+        else bm25_rescore_kernel<<<n_queries, kRsThreads, 0, st>>>(p, c, out_scores, out_ids, out_counts);
         EZR_LAUNCH_CHECK();
     }
     return EZR_OK;
@@ -734,6 +760,101 @@ static int check_index(const ezr_bm25_index* ix) {
     EZR_CHECK_ARG(ix->score_type == EZR_F64 || ix->score_type == EZR_F32, "bm25: bad score_type");
     EZR_CHECK_ARG(ix->n_postings >= 0 && ix->n_postings < ((int64_t)1 << 31),
                   "bm25: %lld postings in one index; shard the corpus (limit 2^31-1 per shard)", (long long)ix->n_postings);
+    return EZR_OK;
+}
+
+// ---- score rows in query blocks: k > 32 without the deep form, and the deep form's overflowed queries ----
+// The rows of one block take at most kRowsBudget bytes, so the workspace does not grow with Q * n_docs.  A block's
+// queries (a run of the batch, or entries of a query list) are gathered into a table with two q_ptr entries per
+// query: block query i is table query 2i, which the ordered kernel reaches through its query list, with its terms
+// read from the caller's q_terms, and whose row lands at 2i * n_docs (the odd rows are never written or read).
+constexpr size_t kRowsBudget = (size_t)1 << 30;
+
+__global__ void bm25_rows_gather_kernel(const int32_t* __restrict__ q_ptr, const int32_t* __restrict__ q_group,
+                                        const int32_t* __restrict__ list, int j0, int nb, int32_t* __restrict__ qp,
+                                        int32_t* __restrict__ ql, int32_t* __restrict__ qg, int32_t* __restrict__ cnt) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) *cnt = nb;
+    if (i >= nb) return;
+    const int q = list ? list[j0 + i] : j0 + i;
+    qp[2 * i] = q_ptr[q];
+    qp[2 * i + 1] = q_ptr[q + 1];
+    ql[i] = 2 * i;
+    if (q_group) qg[i] = q_group[q];
+}
+
+template <typename S>
+__global__ void bm25_rows_scatter_kernel(const S* __restrict__ bs, const int32_t* __restrict__ bi,
+                                         const int32_t* __restrict__ bc, const int32_t* __restrict__ list, int j0,
+                                         int k, S* __restrict__ out_s, int32_t* __restrict__ out_i,
+                                         int32_t* __restrict__ out_c) {
+    const int i = blockIdx.x;
+    const int64_t q = list ? list[j0 + i] : j0 + i;
+    for (int t = threadIdx.x; t < k; t += blockDim.x) {
+        out_s[q * k + t] = bs[(int64_t)i * k + t];
+        out_i[q * k + t] = bi[(int64_t)i * k + t];
+    }
+    if (threadIdx.x == 0) out_c[q] = bc[i];
+}
+
+struct RowsWorkspace {
+    void* rows;
+    void* sel;
+    size_t sel_bytes;
+    void* blk_s;
+    int32_t *blk_i, *blk_c, *qp, *ql, *qg, *cnt;
+    int block;
+    size_t total;
+};
+
+static RowsWorkspace rows_carve(void* base, const ezr_bm25_index* ix, int n_queries, int k) {
+    RowsWorkspace w;
+    const bool f64 = ix->score_type == EZR_F64;
+    const size_t ss = f64 ? 8 : 4, nd = (size_t)ix->n_docs;
+    const size_t per = 2 * nd * ss;
+    size_t b = per ? kRowsBudget / per : (size_t)n_queries;
+    b = b < 1 ? 1 : (b > (size_t)n_queries ? (size_t)n_queries : b);
+    w.block = (int)b;
+    w.sel_bytes = 0;                                    // a smaller last block can need more (more parts per row)
+    for (int m = 1; m <= w.block; ++m) {
+        const size_t sb = f64 ? select_rows_ws<double>(m, ix->n_docs, k) : select_rows_ws<float>(m, ix->n_docs, k);
+        if (sb > w.sel_bytes) w.sel_bytes = sb;
+    }
+    char* p = reinterpret_cast<char*>(base);
+    size_t off = 0;
+    w.rows = p + off;   off += align_up((2 * b - 1) * nd * ss, 256);
+    w.sel = p + off;    off += align_up(w.sel_bytes, 256);
+    w.blk_s = p + off;  off += align_up(b * k * ss, 256);
+    w.blk_i = reinterpret_cast<int32_t*>(p + off);  off += align_up(b * k * 4, 256);
+    w.blk_c = reinterpret_cast<int32_t*>(p + off);  off += align_up(b * 4, 256);
+    w.qp = reinterpret_cast<int32_t*>(p + off);     off += align_up(2 * b * 4, 256);
+    w.ql = reinterpret_cast<int32_t*>(p + off);     off += align_up(b * 4, 256);
+    w.qg = reinterpret_cast<int32_t*>(p + off);     off += align_up(b * 4, 256);
+    w.cnt = reinterpret_cast<int32_t*>(p + off);    off += 256;
+    w.total = off;
+    return w;
+}
+
+// top-k of queries list[0 .. n) (list == NULL: queries 0 .. n) from their score rows, block by block
+template <typename S>
+static int rows_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t* q_terms, int k,
+                     const int32_t* q_group, int id_base, const int32_t* list, int n, S* out_s, int32_t* out_ids,
+                     int32_t* out_counts, const RowsWorkspace& w, cudaStream_t st) {
+    for (int j0 = 0; j0 < n; j0 += w.block) {
+        const int nb = n - j0 < w.block ? n - j0 : w.block;
+        bm25_rows_gather_kernel<<<ceil_div(nb, 256), 256, 0, st>>>(q_ptr, q_group, list, j0, nb, w.qp, w.ql, w.qg,
+                                                                   w.cnt);
+        EZR_LAUNCH_CHECK();
+        int rc = bm25_launch<S>(ix, w.qp, q_terms, nb, k, nullptr, 0, 1, w.rows, nullptr, nullptr, st, w.ql, w.cnt);
+        if (rc) return rc;
+        rc = select_rows_impl<S>((const S*)w.rows, nb, ix->n_docs, 2 * ix->n_docs, k, 1, ix->doc_group,
+                                 q_group ? w.qg : nullptr, id_base, (S*)w.blk_s, w.blk_i, w.blk_c, w.sel, w.sel_bytes,
+                                 st);
+        if (rc) return rc;
+        bm25_rows_scatter_kernel<S><<<nb, 256, 0, st>>>((const S*)w.blk_s, w.blk_i, w.blk_c, list, j0, k, out_s,
+                                                        out_ids, out_counts);
+        EZR_LAUNCH_CHECK();
+    }
     return EZR_OK;
 }
 
@@ -856,11 +977,11 @@ size_t ezr_bm25_topk_workspace(const ezr_bm25_index* ix, int32_t n_queries, int3
         if (pk_usable(ix, k)) return lists + pk_carve(nullptr, n_queries).total;
         return lists + align_up((size_t)n_queries * 4, 256);
     }
-    // score rows, one query block at a time is the caller's job: here all rows at once
-    size_t rows = align_up((size_t)n_queries * ix->n_docs * ss, 256);
-    size_t sel = ix->score_type == EZR_F64 ? select_rows_ws<double>(n_queries, ix->n_docs, k)
-                                            : select_rows_ws<float>(n_queries, ix->n_docs, k);
-    return rows + sel;
+    // deep form: candidate lists and their score rows (Q * pk_deep_list_cap(k)), plus one block of score rows for
+    // the queries that overflow them; otherwise blocks of score rows only
+    const size_t rows = rows_carve(nullptr, ix, n_queries, k).total;
+    if (pk_deep_usable(ix, k)) return pk_carve(nullptr, n_queries, pk_deep_list_cap(k), true).total + rows;
+    return rows;
 }
 
 int ezr_bm25_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t* q_terms, int32_t n_queries,
@@ -916,18 +1037,31 @@ int ezr_bm25_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t*
                    : merge_impl<float>((const float*)ps, pi, n_queries, n_cand, n_cand, k, id_base,
                                        (float*)out_scores, out_ids, out_counts, st);
     }
-    void* rows = workspace;
-    void* sel_ws = (char*)workspace + align_up((size_t)n_queries * ix->n_docs * ss, 256);
-    const size_t sel_bytes = workspace_bytes - align_up((size_t)n_queries * ix->n_docs * ss, 256);
-    rc = f64 ? bm25_launch<double>(ix, q_ptr, q_terms, n_queries, k, nullptr, 0, 1, rows, nullptr, nullptr, st)
-             : bm25_launch<float>(ix, q_ptr, q_terms, n_queries, k, nullptr, 0, 1, rows, nullptr, nullptr, st);
-    if (rc) return rc;
-    return f64 ? select_rows_impl<double>((const double*)rows, n_queries, ix->n_docs, ix->n_docs, k, 1,
-                                          ix->doc_group, q_group, id_base, (double*)out_scores, out_ids,
-                                          out_counts, sel_ws, sel_bytes, st)
-               : select_rows_impl<float>((const float*)rows, n_queries, ix->n_docs, ix->n_docs, k, 1,
-                                         ix->doc_group, q_group, id_base, (float*)out_scores, out_ids,
-                                         out_counts, sel_ws, sel_bytes, st);
+    if (pk_deep_usable(ix, k)) {
+        // candidates from packed postings -> exact scores in [Q][cap] rows -> the select takes each top-k;
+        // overflowed queries (normally none) are then answered from their score rows
+        const int cap = pk_deep_list_cap(k);
+        const PkWorkspace w = pk_carve(workspace, n_queries, cap, true);
+        const RowsWorkspace rw = rows_carve((char*)workspace + w.total, ix, n_queries, k);
+        EZR_CUDA(cudaMemsetAsync(workspace, 0, w.zero_bytes, st));
+        rc = pk_launch(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, w, nullptr, nullptr, nullptr, st, true);
+        if (rc) return rc;
+        rc = launch_select<double>(w.rows, w.cand_ids, n_queries, cap, cap, 1, k, 1, nullptr, nullptr, id_base,
+                                   (double*)out_scores, out_ids, out_counts, st);
+        if (rc) return rc;
+        // the host learns how many queries overflowed (one small copy + stream sync) to size the score-row pass
+        int32_t n_ovf = 0;
+        EZR_CUDA(cudaMemcpyAsync(&n_ovf, w.ovf_n, 4, cudaMemcpyDeviceToHost, st));
+        EZR_CUDA(cudaStreamSynchronize(st));
+        if (n_ovf == 0) return EZR_OK;
+        return rows_topk<double>(ix, q_ptr, q_terms, k, q_group, id_base, w.ovf_list, n_ovf, (double*)out_scores,
+                                 out_ids, out_counts, rw, st);
+    }
+    const RowsWorkspace rw = rows_carve(workspace, ix, n_queries, k);
+    return f64 ? rows_topk<double>(ix, q_ptr, q_terms, k, q_group, id_base, nullptr, n_queries, (double*)out_scores,
+                                   out_ids, out_counts, rw, st)
+               : rows_topk<float>(ix, q_ptr, q_terms, k, q_group, id_base, nullptr, n_queries, (float*)out_scores,
+                                  out_ids, out_counts, rw, st);
 }
 
 int ezr_bm25_scores(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t* q_terms, int32_t n_queries,

@@ -71,6 +71,15 @@ constexpr int kPkNeDen = 10;
 #define EZR_BM25_PK_UNROLL 8
 #endif
 constexpr int kPkThreads = EZR_BM25_PK_THREADS;           // candidate-pass CTA (independent of the ordered kernel's)
+// Deep form (32 < k <= 1024): the capacities grow with k.  A (query, range) CTA without a bound keeps the documents
+// within the slack of its exact k-th best sum (k plus ties); with a bound, those crossing it.  Between range chunks
+// the bound kernel cuts every list back to about k, and the next chunk adds about k more (its ranges are compared
+// against the k-th best of all ranges before it).  The first chunk's ranges may all run before any bound exists
+// (small batches): four ranges of k each.  Hence 2k + 512 per (query, range) and 4k + 1024 per query; a query that
+// overflows either is answered from its score row, so results never depend on these numbers.
+__host__ __device__ constexpr int pk_deep_local_cap(int k) { return 2 * k + 512; }
+__host__ __device__ constexpr int pk_deep_list_cap(int k) { return 4 * k + 1024; }
+constexpr int kPkHist = 256 + 4;                          // radix-select bins + broadcast slots (block_kth_largest)
 constexpr int kPkGroup = kPkThreads / 32;                 // lanes per group: 32 disjoint group maxima
 static_assert(kPkThreads % 32 == 0 && kPkThreads >= 64 && (kPkGroup & (kPkGroup - 1)) == 0, "bad EZR_BM25_PK_THREADS");
 static_assert(kBmRange % (4 * kPkThreads) == 0, "range must be a multiple of 4 * EZR_BM25_PK_THREADS");
@@ -157,6 +166,67 @@ __global__ void bm25_plan_kernel(const Bm25Params p, int r_begin, int n_r, int n
     plan[i] = e;
 }
 
+// k-th largest POSITIVE value among val(0) .. val(n-1), equal values counted separately; 0 when fewer than k are
+// positive.  Radix select in shared memory: 8-bit digits from the highest set bit of the largest value down, each
+// pass histograms the values that agree with the digits fixed so far.  sh: kPkHist ints.  Every one of the NT
+// threads calls it (it synchronises); n and k are block-uniform.
+template <int NT, typename F>
+__device__ uint32_t block_kth_largest(F val, const int n, const int k, int* sh) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    if (tid == 0) sh[256] = 0;
+    __syncthreads();
+    uint32_t vmax = 0u;
+    for (int i = tid; i < n; i += NT) vmax = max(vmax, val(i));
+    vmax = __reduce_max_sync(0xffffffffu, vmax);
+    if (lane == 0) atomicMax(reinterpret_cast<unsigned*>(sh + 256), vmax);
+    __syncthreads();
+    const uint32_t top = (uint32_t)sh[256];
+    uint32_t prefix = 0u, mask = 0u;
+    int kk = k;                                          // rank still to find among the values that match prefix
+    int s = max(32 - __clz(top) - 8, 0);
+    for (;;) {
+        for (int i = tid; i < 256; i += NT) sh[i] = 0;
+        __syncthreads();
+        for (int i = tid; i < n; i += NT) {
+            const uint32_t v = val(i);
+            if (v != 0u && (v & mask) == prefix) atomicAdd(&sh[(v >> s) & 255u], 1);
+        }
+        __syncthreads();
+        if (tid < 32) {                                  // lane l holds bins 255-8l .. 248-8l (descending)
+            int c[8], sum = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { c[j] = sh[255 - 8 * lane - j]; sum += c[j]; }
+            int inc = sum;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, inc, o);
+                if (lane >= o) inc += v;
+            }
+            int above = inc - sum;
+            if (above < kk && kk <= inc) {               // exactly one lane: the digit of the k-th value is here
+                int d = -1, a = 0;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    if (d < 0 && above + c[j] >= kk) { d = 255 - 8 * lane - j; a = above; }
+                    above += c[j];
+                }
+                sh[257] = d;
+                sh[258] = a;
+            }
+            if (lane == 31 && inc < kk) sh[257] = -1;    // fewer than k positive values (first pass only)
+        }
+        __syncthreads();
+        const int d = sh[257], above = sh[258];
+        __syncthreads();                                 // the bins and slots are rewritten by the next pass
+        if (d < 0) return 0u;
+        prefix = (prefix & ~(255u << s)) | ((uint32_t)d << s);
+        mask |= 255u << s;
+        kk -= above;
+        if (s == 0) return prefix;
+        s = max(s - 8, 0);                               // the last pass may overlap fixed bits: they match prefix
+    }
+}
+
 // ---- phase 1 ----
 // One CTA per (query, document range).  Work is dealt to warps in pieces of kPkPiece postings (256 by default) over
 // ALL terms of the query (a warp's lanes each hold one term's segment; ballot + shuffles map a piece number to its
@@ -166,12 +236,22 @@ constexpr int kPkWarps = kPkThreads / 32;
 constexpr int kPkUnroll = EZR_BM25_PK_UNROLL;                             // loads a lane keeps in flight
 constexpr int kPkPiece = 32 * kPkUnroll;                 // postings per work item
 
-__global__ void __launch_bounds__(kPkThreads, EZR_BM25_PK_MINB)
+// DEEP (32 < k <= 1024): the first bound of a range is its exact k-th best sum (block_kth_largest over the
+// accumulators), the candidate list lives in dynamic shared memory behind the accumulators, the capacities are
+// pk_deep_local_cap / pk_deep_list_cap, and the in-range raise is a select over the range's candidates.  (A kernel
+// template, not a body inlined into two kernels: inlining changes the k <= 32 instance's register allocation.)
+template <bool DEEP>
+__global__ void __launch_bounds__(kPkThreads, DEEP ? 4 : EZR_BM25_PK_MINB)
 bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
     extern __shared__ __align__(16) unsigned char pk_smem_raw[];
     uint32_t* acc = reinterpret_cast<uint32_t*>(pk_smem_raw);   // [kBmRange + 32] integer upper-bound scores + spare
-    __shared__ int s_wi[kPkLocalCap];
+    __shared__ int s_wi_fixed[DEEP ? 1 : kPkLocalCap];
     __shared__ int s_cnt, s_b, s_thr;
+    // DEEP: [kBmRange + 32] accumulators | [kPkHist] select scratch | [pk_deep_local_cap(k)] candidate list
+    int* s_hist = reinterpret_cast<int*>(acc + kBmRange + 32);
+    int* s_wi = DEEP ? s_hist + kPkHist : s_wi_fixed;
+    const int local_cap = DEEP ? pk_deep_local_cap(p.k) : kPkLocalCap;
+    const int list_cap = DEEP ? pk_deep_list_cap(p.k) : kPkListCap;
 
     const int q = blockIdx.x, r = r_begin + blockIdx.y;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -250,7 +330,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
         const uint32_t dl = x >> kPkWBits;
         if (want == -1 || p.doc_group[rbase + (int)dl] == want) {
             const int idx = atomicAdd(&s_cnt, 1);
-            if (idx < kPkLocalCap) s_wi[idx] = (int)dl;
+            if (idx < local_cap) s_wi[idx] = (int)dl;
         }
     };
     for (int tb = 0; tb < m; tb += 32) {
@@ -319,7 +399,23 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
         // No bound yet (first ranges of a query): k-th largest of 32 disjoint group maxima = G, then compact.
         constexpr int kPer = kBmRange / kPkThreads;
         uint32_t tmax = 0u;
-        if (want == -1) {
+        if constexpr (DEEP) {
+            // G = the exact k-th best sum of the range's documents in the query's group (the others are zeroed
+            // first; the documents past n_docs hold 0 and never reach doc_group)
+            if (want != -1) {
+#pragma unroll 4
+                for (int i = 0; i < kPer; ++i) {
+                    const int doc = tid + i * kPkThreads;
+                    if (acc[doc] != 0u && p.doc_group[rbase + doc] != want) acc[doc] = 0u;
+                }
+                __syncthreads();
+            }
+#pragma unroll
+            for (int i = 0; i < kPer; ++i) tmax = max(tmax, acc[tid + i * kPkThreads]);
+            const uint32_t kth = block_kth_largest<kPkThreads>([&](int i) { return acc[i]; }, kBmRange, p.k, s_hist);
+            if (tid == 0) s_thr = (int)kth;
+            __syncthreads();
+        } else if (want == -1) {
 #pragma unroll
             for (int i = 0; i < kPer; ++i) tmax = max(tmax, acc[tid + i * kPkThreads]);
         } else {
@@ -330,23 +426,25 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
                 if (v > tmax && p.doc_group[rbase + doc] == want) tmax = v;
             }
         }
-        uint32_t gmax = tmax;
+        if constexpr (!DEEP) {
+            uint32_t gmax = tmax;
 #pragma unroll
-        for (int o = kPkGroup / 2; o > 0; o >>= 1) gmax = max(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
-        if ((lane & (kPkGroup - 1)) == 0) s_wi[tid / kPkGroup] = (int)gmax;
-        if (tid == 0) s_thr = 0;
-        __syncthreads();
-        if (warp == 0) {
-            const int mine = s_wi[lane];
-            int rank = 0;
+            for (int o = kPkGroup / 2; o > 0; o >>= 1) gmax = max(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
+            if ((lane & (kPkGroup - 1)) == 0) s_wi[tid / kPkGroup] = (int)gmax;
+            if (tid == 0) s_thr = 0;
+            __syncthreads();
+            if (warp == 0) {
+                const int mine = s_wi[lane];
+                int rank = 0;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                const int o = s_wi[j];
-                rank += (o > mine || (o == mine && j < lane)) ? 1 : 0;
+                for (int j = 0; j < 32; ++j) {
+                    const int o = s_wi[j];
+                    rank += (o > mine || (o == mine && j < lane)) ? 1 : 0;
+                }
+                if (rank == p.k - 1) s_thr = mine;       // 0 when fewer than k groups hold a positive score
             }
-            if (rank == p.k - 1) s_thr = mine;           // 0 when fewer than k groups hold a positive score
+            __syncthreads();
         }
-        __syncthreads();
         const int g = s_thr;
         const int bl = g > 0 ? g - slack : 0;            // B from this range alone
         const uint32_t tl = (uint32_t)max(bl - 1, 1);
@@ -357,7 +455,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
                 const int doc = tid + i * kPkThreads;
                 if (acc[doc] >= tl && (want == -1 || p.doc_group[rbase + doc] == want)) {
                     const int idx = atomicAdd(&s_cnt, 1);
-                    if (idx < kPkLocalCap) s_wi[idx] = doc;
+                    if (idx < local_cap) s_wi[idx] = doc;
                 }
             }
         }
@@ -366,7 +464,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
     }
     const int n = s_cnt;
     if (n == 0) return;
-    if (n > kPkLocalCap) {
+    if (n > local_cap) {
         if (tid == 0) c.ovf[q] = 1;
         return;
     }
@@ -403,56 +501,83 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
         const uint32_t mine = acc[dl];
         if (nm != 0u && (int)mine < bound - 1) continue;  // crossed only the relaxed threshold
         const int slot = atomicAdd(c.cand_cnt + q, 1);
-        if (slot < kPkListCap) {
-            c.cand_ids[(int64_t)q * kPkListCap + slot] = rbase + dl;
-            c.cand_q[(int64_t)q * kPkListCap + slot] = (int)mine;
-            c.cand_u[(int64_t)q * kPkListCap + slot] = (int)mine;       // full sums: lower and upper bound coincide
+        if (slot < list_cap) {
+            c.cand_ids[(int64_t)q * list_cap + slot] = rbase + dl;
+            c.cand_q[(int64_t)q * list_cap + slot] = (int)mine;
+            c.cand_u[(int64_t)q * list_cap + slot] = (int)mine;       // full sums: lower and upper bound coincide
         } else {
             c.ovf[q] = 1;
         }
-        if (track && n >= p.k) {                         // this range alone holds k documents above the bound
-            int rank = 0;
-            for (int j = 0; j < n; ++j) {
-                const uint32_t o = acc[s_wi[j]];
-                rank += (o > mine || (o == mine && j < i)) ? 1 : 0;
+        if constexpr (!DEEP) {
+            if (track && n >= p.k) {                     // this range alone holds k documents above the bound
+                int rank = 0;
+                for (int j = 0; j < n; ++j) {
+                    const uint32_t o = acc[s_wi[j]];
+                    rank += (o > mine || (o == mine && j < i)) ? 1 : 0;
+                }
+                if (rank == p.k - 1 && (int)mine - slack > bound) atomicMax(c.thr_q + q, (int)mine - slack);
             }
-            if (rank == p.k - 1 && (int)mine - slack > bound) atomicMax(c.thr_q + q, (int)mine - slack);
+        }
+    }
+    if constexpr (DEEP) {
+        if (track && n >= p.k) {                         // block-uniform: the same raise, by a select
+            __syncthreads();                             // relaxed crossers were dropped above, acc is final
+            const int kth = (int)block_kth_largest<kPkThreads>([&](int i) { return acc[s_wi[i]]; }, n, p.k, s_hist);
+            if (tid == 0 && kth - slack > bound) atomicMax(c.thr_q + q, kth - slack);
         }
     }
 }
+
+
+inline size_t pk_deep_cand_smem(int k) { return (size_t)(kBmRange + 32 + kPkHist + pk_deep_local_cap(k)) * 4; }
 
 // ---- between range chunks: raise every query's bound to the k-th best of ALL candidates so far, drop the rest ----
 // (a single range only knows its own k-th best; the bound that keeps later ranges quiet is the running global one)
 constexpr int kBdThreads = 128;
 
-__global__ void __launch_bounds__(kBdThreads)
-bm25_bound_kernel(const Bm25Params p, const PkParams c) {
-    __shared__ int s_q[kPkListCap];
-    __shared__ int s_u[kPkListCap];
-    __shared__ int s_id[kPkListCap];
+// DEEP: the list has pk_deep_list_cap(k) slots, staged in dynamic shared memory, and the k-th largest lower bound
+// comes from a radix select instead of pairwise ranks.
+template <bool DEEP>
+__device__ __forceinline__ void bm25_bound_body(const Bm25Params& p, const PkParams& c) {
+    __shared__ int s_q_fixed[DEEP ? 1 : kPkListCap];
+    __shared__ int s_u_fixed[DEEP ? 1 : kPkListCap];
+    __shared__ int s_id_fixed[DEEP ? 1 : kPkListCap];
     __shared__ int s_kth, s_n2;
+    extern __shared__ __align__(16) unsigned char pk_smem_raw[];
+    const int list_cap = DEEP ? pk_deep_list_cap(p.k) : kPkListCap;
+    // DEEP: [kPkHist] select scratch | s_q | s_u | s_id, list_cap each
+    int* s_hist = reinterpret_cast<int*>(pk_smem_raw);
+    int* s_q = DEEP ? s_hist + kPkHist : s_q_fixed;
+    int* s_u = DEEP ? s_hist + kPkHist + list_cap : s_u_fixed;
+    int* s_id = DEEP ? s_hist + kPkHist + 2 * list_cap : s_id_fixed;
     const int q = blockIdx.x, tid = threadIdx.x;
     const int n = c.cand_cnt[q];
     if (c.ovf[q] != 0 || n < p.k) return;                // block-uniform
-    if (n > kPkListCap) {
+    if (n > list_cap) {
         if (tid == 0) c.ovf[q] = 1;
         return;
     }
     for (int i = tid; i < n; i += kBdThreads) {
-        s_q[i] = c.cand_q[(int64_t)q * kPkListCap + i];
-        s_u[i] = c.cand_u[(int64_t)q * kPkListCap + i];
-        s_id[i] = c.cand_ids[(int64_t)q * kPkListCap + i];
+        s_q[i] = c.cand_q[(int64_t)q * list_cap + i];
+        s_u[i] = c.cand_u[(int64_t)q * list_cap + i];
+        s_id[i] = c.cand_ids[(int64_t)q * list_cap + i];
     }
     if (tid == 0) s_n2 = 0;
     __syncthreads();
-    for (int i = tid; i < n; i += kBdThreads) {
-        const int mine = s_q[i];
-        int rank = 0;
-        for (int j = 0; j < n; ++j) {
-            const int o = s_q[j];
-            rank += (o > mine || (o == mine && j < i)) ? 1 : 0;
+    if constexpr (DEEP) {
+        // lower bounds are >= 1 (candidates pass a threshold of at least 1), so the select sees all n of them
+        const int kth = (int)block_kth_largest<kBdThreads>([&](int i) { return (uint32_t)s_q[i]; }, n, p.k, s_hist);
+        if (tid == 0) s_kth = kth;
+    } else {
+        for (int i = tid; i < n; i += kBdThreads) {
+            const int mine = s_q[i];
+            int rank = 0;
+            for (int j = 0; j < n; ++j) {
+                const int o = s_q[j];
+                rank += (o > mine || (o == mine && j < i)) ? 1 : 0;
+            }
+            if (rank == p.k - 1) s_kth = mine;           // ranks are a permutation: exactly one writer
         }
-        if (rank == p.k - 1) s_kth = mine;               // ranks are a permutation: exactly one writer
     }
     __syncthreads();
     const int qs = p.q_ptr[q];
@@ -461,9 +586,9 @@ bm25_bound_kernel(const Bm25Params p, const PkParams c) {
     for (int i = tid; i < n; i += kBdThreads) {
         if (s_u[i] >= b - 1) {                           // keep what may still reach it: UPPER bounds decide
             const int pos = atomicAdd(&s_n2, 1);
-            c.cand_q[(int64_t)q * kPkListCap + pos] = s_q[i];
-            c.cand_u[(int64_t)q * kPkListCap + pos] = s_u[i];
-            c.cand_ids[(int64_t)q * kPkListCap + pos] = s_id[i];
+            c.cand_q[(int64_t)q * list_cap + pos] = s_q[i];
+            c.cand_u[(int64_t)q * list_cap + pos] = s_u[i];
+            c.cand_ids[(int64_t)q * list_cap + pos] = s_id[i];
         }
     }
     __syncthreads();
@@ -507,22 +632,38 @@ bm25_bound_kernel(const Bm25Params p, const PkParams c) {
     }
 }
 
+__global__ void __launch_bounds__(kBdThreads)
+bm25_bound_kernel(const Bm25Params p, const PkParams c) {
+    bm25_bound_body<false>(p, c);
+}
+
+__global__ void __launch_bounds__(kBdThreads)
+bm25_bound_deep_kernel(const Bm25Params p, const PkParams c) {
+    bm25_bound_body<true>(p, c);
+}
+
+inline size_t pk_deep_bound_smem(int k) { return (size_t)(kPkHist + 3 * pk_deep_list_cap(k)) * 4; }
+
 // ---- phase 2: exact scores of the candidates in token order, canonical top-k ----
 constexpr int kRsThreads = 128;
 constexpr int kRsTok = 64;     // tokens whose (term, base) are staged in shared memory
 constexpr int kRsU = 4;        // candidates a warp scores at once (independent binary searches in flight)
 
-__global__ void __launch_bounds__(kRsThreads)
-bm25_rescore_kernel(const Bm25Params p, const PkParams c, double* __restrict__ out_scores,
-                    int32_t* __restrict__ out_ids, int32_t* __restrict__ out_counts) {
-    __shared__ double s_sc[kPkListCap];
-    __shared__ int s_id[kPkListCap];
+// DEEP: out_scores is a [Q][pk_deep_list_cap(k)] row of exact scores beside the candidate ids (ids past the
+// query's candidates set to -1), from which the caller's select takes the canonical top-k.
+template <bool DEEP>
+__device__ __forceinline__ void bm25_rescore_body(const Bm25Params& p, const PkParams& c,
+                                                  double* __restrict__ out_scores, int32_t* __restrict__ out_ids,
+                                                  int32_t* __restrict__ out_counts) {
+    __shared__ double s_sc[DEEP ? 1 : kPkListCap];
+    __shared__ int s_id[DEEP ? 1 : kPkListCap];
     __shared__ int s_t[kRsTok];
     __shared__ int s_base[kRsTok];
     __shared__ int s_pos;
+    const int list_cap = DEEP ? pk_deep_list_cap(p.k) : kPkListCap;
     const int q = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n = c.cand_cnt[q];
-    if (c.ovf[q] != 0 || n > kPkListCap) {               // block-uniform
+    if (c.ovf[q] != 0 || n > list_cap) {                 // block-uniform
         if (tid == 0) c.ovf_list[atomicAdd(c.ovf_n, 1)] = q;
         return;
     }
@@ -545,7 +686,7 @@ bm25_rescore_kernel(const Bm25Params p, const PkParams c, double* __restrict__ o
         double s[kRsU];
 #pragma unroll
         for (int u = 0; u < kRsU; ++u) {
-            doc[u] = cb + u < n ? c.cand_ids[(int64_t)q * kPkListCap + cb + u] : -1;
+            doc[u] = cb + u < n ? c.cand_ids[(int64_t)q * list_cap + cb + u] : -1;
             s[u] = 0.0;
         }
         for (int c0 = 0; c0 < m; c0 += 32) {
@@ -602,9 +743,17 @@ bm25_rescore_kernel(const Bm25Params p, const PkParams c, double* __restrict__ o
         }
         if (lane == 0) {
 #pragma unroll
-            for (int u = 0; u < kRsU; ++u)
-                if (cb + u < n) { s_sc[cb + u] = s[u]; s_id[cb + u] = doc[u]; }
+            for (int u = 0; u < kRsU; ++u) {
+                if (cb + u < n) {
+                    if constexpr (DEEP) out_scores[(int64_t)q * list_cap + cb + u] = s[u];
+                    else { s_sc[cb + u] = s[u]; s_id[cb + u] = doc[u]; }
+                }
+            }
         }
+    }
+    if constexpr (DEEP) {
+        for (int i = n + tid; i < list_cap; i += kRsThreads) c.cand_ids[(int64_t)q * list_cap + i] = -1;
+        return;
     }
     __syncthreads();
     for (int i = tid; i < n; i += kRsThreads) {
@@ -627,6 +776,17 @@ bm25_rescore_kernel(const Bm25Params p, const PkParams c, double* __restrict__ o
         out_ids[(int64_t)q * p.k + i] = -1;
     }
     if (tid == 0) out_counts[q] = have;
+}
+
+__global__ void __launch_bounds__(kRsThreads)
+bm25_rescore_kernel(const Bm25Params p, const PkParams c, double* __restrict__ out_scores,
+                    int32_t* __restrict__ out_ids, int32_t* __restrict__ out_counts) {
+    bm25_rescore_body<false>(p, c, out_scores, out_ids, out_counts);
+}
+
+__global__ void __launch_bounds__(kRsThreads)
+bm25_rescore_deep_kernel(const Bm25Params p, const PkParams c, double* __restrict__ rows) {
+    bm25_rescore_body<true>(p, c, rows, nullptr, nullptr);
 }
 
 }  // namespace ezr

@@ -156,7 +156,13 @@ int ezr_bm25_cand_capacity(void);
  * Only documents with score > 0 qualify (retrievers.py:195-196); q_group[i] >= 0 additionally requires
  * doc_group[d] == q_group[i] (filter_dict, retrievers.py:198-202); -1 = no filter.
  * Outputs: out_scores[Q*k] (double/float per index->score_type), out_ids[Q*k] (-1 padded), out_counts[Q].
- * k <= 32 runs fused (accumulators never leave shared memory); larger k (<=1024) goes through a score row. */
+ * k <= 32 runs fused (accumulators never leave shared memory).  32 < k <= 1024 on a float64 index with non-negative
+ * weights and packed postings runs the deep form of the two-phase path: its candidate lists hold 4k + 1024 entries
+ * per query, and a query that overflows them (or one list of 2k + 512 for a range of 8192 documents) is answered
+ * from its score row.  That path reads the number of such queries back to the host once per call (a 4-byte copy
+ * and a stream synchronisation), so it cannot be captured into a CUDA graph.  Every other k > 32 case takes the
+ * top-k from score rows computed in blocks of queries whose rows stay within 1 GiB.
+ * ezr_bm25_topk_workspace therefore grows with Q * k for every index type (plus that one block of score rows). */
 size_t ezr_bm25_topk_workspace(const ezr_bm25_index* index, int32_t n_queries, int32_t k);
 int ezr_bm25_topk(const ezr_bm25_index* index, const int32_t* q_ptr, const int32_t* q_terms, int32_t n_queries,
                   int32_t k, const int32_t* q_group, int32_t id_base, void* out_scores, int32_t* out_ids,
@@ -447,7 +453,8 @@ typedef enum ezr_prof_slot {
     EZR_PROF_DENSE_S8_RESCORE = 11, /* dense_s8_rescore_kernel (exact rescoring + top-k of the candidates) */
     EZR_PROF_DENSE_S8_FULL = 12,    /* full scan of overflowed queries / k > 16 (gather + score rows + select) */
     EZR_PROF_DENSE_WIDE = 13,       /* gemm_wgmma_kernel's score-row instance (form 6; the select counts as merge) */
-    EZR_PROF_COUNT = 14
+    EZR_PROF_BM25_BOUND = 14,       /* bm25_bound_kernel between candidate chunks (also inside EZR_PROF_BM25_CAND) */
+    EZR_PROF_COUNT = 15
 } ezr_prof_slot;
 /* kernels launched by this library since it was loaded (every launch site counts itself) */
 long long ezr_launch_count(void);
