@@ -70,6 +70,7 @@ SIGNATURES = {
     "ezr_merge_topk_workspace": (_sz, [_i32, _i32, _i32, _i32]),
     "ezr_merge_topk": (C.c_int, [_p, _p, _i32, _i32, _i32, _i64, _i32, _p, _p, _p, _p, _sz, _p]),
     "ezr_merge_topk_parts": (C.c_int, [_p, _p, _i32, _i32, _i32, _i64, _i32, _i64, _i32, _p, _p, _p, _p]),
+    "ezr_merge_sorted_parts": (C.c_int, [_p, _p, _i32, _i32, _i32, _i64, _i32, _i64, _i32, _p, _p, _p, _i64, _p]),
     "ezr_dense_topk_workspace": (_sz, [_i64, _i32, _i32, _i32]),
     "ezr_dense_topk": (C.c_int, [_p, _i64, _i32, _i64, _p, _i32, _i64, _i32, _p, _p, _i32, _p, _p, _p, _p, _sz, _p]),
     "ezr_normalize_rows": (C.c_int, [_p, _i32, _i64, _i64, _i32, _p, _i64, _p]),

@@ -200,6 +200,32 @@ def merge_topk_parts(cand_scores: torch.Tensor, cand_ids: torch.Tensor, n_parts:
     return out
 
 
+def merge_sorted_parts(cand_scores: torch.Tensor, cand_ids: torch.Tensor, n_parts: int, part_stride_bytes: int,
+                       k: int, out: Optional[TopK] = None, stream=None) -> TopK:
+    """:func:`merge_topk_parts` for k <= 1024, over parts that are each in canonical order up to their first id < 0
+    (what every route writes) with ids distinct across parts (disjoint shards): ``ezr_merge_sorted_parts``.
+
+    ``out``: result buffers whose rows may be wider than ``k`` (``out.ids.shape[1]`` = the row stride); the slots past
+    each row's count get id -1 and score -inf, so two routes of different depths can share one width."""
+    L = _lib.lib()
+    dev = cand_scores.device
+    assert cand_scores.shape == cand_ids.shape and cand_scores.stride(1) == 1 and cand_ids.stride(1) == 1
+    assert cand_ids.dtype == torch.int32 and cand_scores.stride(0) == cand_ids.stride(0)
+    st = _lib.F64 if cand_scores.dtype == torch.float64 else _lib.F32
+    nq, c = cand_scores.shape
+    if out is None:
+        out = TopK(torch.empty(nq, k, dtype=cand_scores.dtype, device=dev),
+                   torch.empty(nq, k, dtype=torch.int32, device=dev), torch.empty(nq, dtype=torch.int32, device=dev))
+    assert out.scores.dtype == cand_scores.dtype and out.ids.dtype == torch.int32 and out.ids.shape[0] == nq
+    assert out.scores.shape == out.ids.shape and out.scores.is_contiguous() and out.ids.is_contiguous()
+    with torch.cuda.device(dev):
+        _lib.check(L.ezr_merge_sorted_parts(_lib.ptr(cand_scores), _lib.ptr(cand_ids), st, nq, c,
+                                            cand_scores.stride(0), n_parts, part_stride_bytes, k, _lib.ptr(out.scores),
+                                            _lib.ptr(out.ids), _lib.ptr(out.counts), out.ids.shape[1],
+                                            _lib.stream_ptr(stream)), "ezr_merge_sorted_parts")
+    return out
+
+
 def merge_topk(cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int, stream=None) -> TopK:
     """Merge candidate lists [Q, C] (id < 0 = empty) into the canonical top-k."""
     L = _lib.lib()

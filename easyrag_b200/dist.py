@@ -7,7 +7,9 @@ computes its local dense and BM25 top-k with *global* ids straight into one byte
 SINGLE all-gather (NCCL over NVLink on GPUs, gloo in the CPU tests) exchanges the records;
 every rank then merges G*k candidates per route under the canonical order -- the same order
 the 1-GPU path uses, hence identical rank lists -- reading the gathered buffer in place, and
-runs RRF.
+runs RRF.  ``hybrid`` / ``submit`` merge lists of k <= 32 (``ezr_merge_topk_parts``);
+``pipeline_hybrid`` and :class:`ShardedDualSparseRanker` run the pipeline's depths (k <= 1024 per route) and merge the
+sorted per-shard lists by rank (``ezr_merge_sorted_parts``).
 
 Fine ranking (:class:`ShardedCrossEncoderReranker`) splits the other way: every rank holds the whole cross-encoder and
 the same candidate lists, the (query, candidate) pairs are cut into token-balanced runs, one per rank, and ONE
@@ -37,25 +39,37 @@ def shard_bounds(n_rows: int, world: int, rank: int, align: int = 1) -> Tuple[in
     return min(n_rows, lo_u * align), min(n_rows, hi_u * align)
 
 
+def _packed(sizes):
+    """Offsets of arrays of ``sizes`` bytes placed back to back, each at a 16-byte boundary -> (offsets, total)."""
+    o, out = 0, []
+    for s in sizes:
+        out.append(o)
+        o += (s + 15) // 16 * 16
+    return out, o
+
+
 @dataclass
 class RecordLayout:
-    """Byte layout of one rank's contribution: dense scores f32 | dense ids i32 | sparse scores | sparse ids i32."""
+    """Byte layout of one rank's contribution: dense scores f32 | dense ids i32 | sparse scores | sparse ids i32.
+
+    The dense arrays are [Q, k], the sparse ones [Q, k_sparse] (``None``: the same k)."""
     n_queries: int
     k: int
     sparse_bytes: int      # 8 for BM25Okapi (float64), 4 for bm25s (float32)
+    k_sparse: Optional[int] = None
+
+    @property
+    def ks(self) -> int:
+        return self.k if self.k_sparse is None else self.k_sparse
 
     @property
     def sizes(self):
-        n = self.n_queries * self.k
-        return (n * 4, n * 4, n * self.sparse_bytes, n * 4)
+        n, ns = self.n_queries * self.k, self.n_queries * self.ks
+        return (n * 4, n * 4, ns * self.sparse_bytes, ns * 4)
 
     @property
     def offsets(self):
-        o, out = 0, []
-        for s in self.sizes:
-            out.append(o)
-            o += (s + 15) // 16 * 16
-        return out, o
+        return _packed(self.sizes)
 
     @property
     def nbytes(self) -> int:
@@ -63,16 +77,36 @@ class RecordLayout:
 
 
 def record_views(layout: RecordLayout, buf: torch.Tensor):
-    """The four per-route arrays of one rank's record as typed [Q, k] views of the byte buffer ``buf``
-    (dense scores f32, dense ids i32, sparse scores f64/f32, sparse ids i32): writing through them fills the
-    message in place, reading them from a gathered buffer needs no unpacking."""
+    """The four per-route arrays of one rank's record as typed views of the byte buffer ``buf`` (dense scores f32
+    and ids i32 [Q, k], sparse scores f64/f32 and ids i32 [Q, k_sparse]): writing through them fills the message in
+    place, reading them from a gathered buffer needs no unpacking."""
     offs, _ = layout.offsets
-    q, k = layout.n_queries, layout.k
+    q, k, ks = layout.n_queries, layout.k, layout.ks
     sdt = torch.float64 if layout.sparse_bytes == 8 else torch.float32
     out = []
-    for off, size, dt in zip(offs, layout.sizes, (torch.float32, torch.int32, sdt, torch.int32)):
-        out.append(buf[off:off + size].view(dt).view(q, k))
+    for off, size, dt, w in zip(offs, layout.sizes, (torch.float32, torch.int32, sdt, torch.int32), (k, k, ks, ks)):
+        out.append(buf[off:off + size].view(dt).view(q, w))
     return out
+
+
+MAX_DEEP_K = 1024          # per-route depth of the deep merge (ezr_merge_sorted_parts)
+
+
+def _check_depth(name: str, k: int) -> None:
+    if not 1 <= k <= MAX_DEEP_K:
+        raise ValueError(f"{name}={k} out of [1, {MAX_DEEP_K}]")
+
+
+def _merged(nq: int, width: int, score_dtype, dev):
+    """A [Q, width] result buffer of the deep merge (rows wider than a route's k are padded with id -1)."""
+    from .batched import TopK
+    return TopK(torch.empty(nq, width, dtype=score_dtype, device=dev), torch.empty(nq, width, dtype=torch.int32, device=dev),
+                torch.empty(nq, dtype=torch.int32, device=dev))
+
+
+def _narrow(t, k: int):
+    from .batched import TopK
+    return TopK(t.scores[:, :k], t.ids[:, :k], t.counts)
 
 
 class ShardedCoarseRanker:
@@ -168,6 +202,122 @@ class ShardedCoarseRanker:
 
     def join(self) -> None:
         self.ranker.join()
+
+    def pipeline_hybrid(self, queries, q_ptr, q_terms, k_dense: int = 288, k_sparse: int = 192, k_out: int = 256,
+                        K: int = 60, q_group=None, canon: Optional[torch.Tensor] = None):
+        """dense top-``k_dense`` + BM25 top-``k_sparse`` + RRF to ``k_out`` at the pipeline's depths (pipeline.py's
+        f_topk_1 / f_topk_2 / f_topk), each route k in [1, 1024] -> (fused, sparse, dense), bit-identical to one GPU
+        running ``dense_topk(k_dense)`` + ``bm25_topk(k_sparse)`` + ``fuse_lists`` over the whole corpus.
+
+        Both routes run on the caller's stream and write straight into one record (:class:`RecordLayout` with
+        ``k_sparse``); ONE ``all_gather_into_tensor`` exchanges it; ``ezr_merge_sorted_parts`` merges each route's G
+        sorted lists in place into a [Q, W] buffer, W = max(k_dense, k_sparse), the one width the RRF kernel takes.
+        ``sparse`` / ``dense`` are [Q, k] views of those buffers.  Buffers are allocated once per shape.
+
+        Memory: the gathered buffer holds G * Q * (8 * k_dense + (S + 4) * k_sparse) bytes, S the BM25 score size (8
+        for Okapi, 4 for bm25s): 369 MB at G = 8, Q = 10k, 288 / 192, float64.  Batches are not split into query
+        blocks, so a very large Q needs the caller to split it."""
+        from . import batched
+        _check_depth("k_dense", k_dense)
+        _check_depth("k_sparse", k_sparse)
+        if k_out < 1:
+            raise ValueError(f"k_out={k_out} must be >= 1")
+        r = self.ranker
+        nq = queries.shape[0]
+        key = ("deep", nq, k_dense, k_sparse, k_out)
+        if key not in self._state:
+            dev, sdt = r.device, r.sparse.score_dtype
+            layout = RecordLayout(nq, k_dense, 8 if sdt == torch.float64 else 4, k_sparse=k_sparse)
+            record = torch.zeros(layout.nbytes, dtype=torch.uint8, device=dev)
+            gathered = torch.zeros(self.world * layout.nbytes, dtype=torch.uint8, device=dev)
+            ds, di, ss, si = record_views(layout, record)
+            cnt = lambda: torch.empty(nq, dtype=torch.int32, device=dev)
+            width = max(k_dense, k_sparse)
+            self._state[key] = dict(
+                layout=layout, record=record, gathered=gathered,
+                d_local=batched.TopK(ds, di, cnt()), s_local=batched.TopK(ss, si, cnt()),
+                views=record_views(layout, gathered[:layout.nbytes]),
+                dense=_merged(nq, width, torch.float32, dev), sparse=_merged(nq, width, sdt, dev),
+                fused=_merged(nq, k_out, torch.float64, dev))
+        st = self._state[key]
+        batched.bm25_topk(r.sparse, q_ptr, q_terms, k_sparse, q_group=q_group, ws=r.ws_sparse, out=st["s_local"])
+        batched.dense_topk(r.dense, queries, k_dense, q_group=q_group, ws=r.ws_dense, out=st["d_local"])
+        dist.all_gather_into_tensor(st["gathered"], st["record"], group=self.group)   # the one collective
+        g_ds, g_di, g_ss, g_si = st["views"]
+        nbytes = st["layout"].nbytes
+        dense = batched.merge_sorted_parts(g_ds, g_di, self.world, nbytes, k_dense, out=st["dense"])
+        sparse = batched.merge_sorted_parts(g_ss, g_si, self.world, nbytes, k_sparse, out=st["sparse"])
+        fused = batched.rrf_fuse(sparse.ids, sparse.counts, dense.ids, dense.counts, k_out, K=K,
+                                 canon=canon if canon is not None else r.canon, out=st["fused"])
+        return fused, _narrow(sparse, k_sparse), _narrow(dense, k_dense)
+
+
+class ShardedDualSparseRanker:
+    """``batched.dual_sparse_fusion`` over a row-sharded corpus (the reference's default coarse ranker, pipeline.py:
+    357-365: chunk-text BM25 top-k_chunk + knowledge-path BM25 top-k_path + ``HybridRetriever.fusion``); every rank
+    returns the full result, bit-identical to ``dual_sparse_fusion`` over the unsharded indexes.
+
+    Both indexes are this rank's shard (``doc_lo`` / ``doc_hi``, corpus-global statistics, global ids).  The two
+    lists go into one record, ONE ``all_gather_into_tensor`` exchanges it, ``ezr_merge_sorted_parts`` merges each
+    list's G sorted parts in place, and ``ezr_fusion_simple`` fuses the merged lists.  Record and gather buffers are
+    allocated once per shape; the gathered buffer holds G * Q * (S_c + 4) * k_chunk + G * Q * (S_p + 4) * k_path bytes
+    (S the score size of each index: 8 for Okapi, 4 for bm25s)."""
+
+    def __init__(self, chunk_index, path_index, canon: Optional[torch.Tensor] = None, group=None):
+        from .batched import Workspace
+        assert chunk_index.device == path_index.device
+        self.chunk, self.path = chunk_index, path_index
+        self.device = chunk_index.device
+        self.canon = None if canon is None else canon.to(device=self.device, dtype=torch.int32).contiguous()
+        self.group = group
+        self.world = dist.get_world_size(group)
+        self.rank = dist.get_rank(group)
+        self.ws = Workspace(self.device)
+        self._state = {}
+
+    def _make(self, nq: int, k_chunk: int, k_path: int):
+        from .batched import TopK
+        dev = self.device
+        dts = (self.chunk.score_dtype, torch.int32, self.path.score_dtype, torch.int32)
+        shapes = ((nq, k_chunk), (nq, k_chunk), (nq, k_path), (nq, k_path))
+        sizes = [q * k * torch.empty(0, dtype=dt).element_size() for (q, k), dt in zip(shapes, dts)]
+        offs, nbytes = _packed(sizes)
+        record = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+        gathered = torch.zeros(self.world * nbytes, dtype=torch.uint8, device=dev)
+
+        def views(buf):
+            return [buf[o:o + s].view(dt).view(*shp) for o, s, dt, shp in zip(offs, sizes, dts, shapes)]
+        cs, ci, ps, pi = views(record)
+        cnt = lambda: torch.empty(nq, dtype=torch.int32, device=dev)
+        width = max(k_chunk, k_path)
+        return dict(nbytes=nbytes, record=record, gathered=gathered, c_local=TopK(cs, ci, cnt()),
+                    p_local=TopK(ps, pi, cnt()), views=views(gathered[:nbytes]),
+                    chunk=_merged(nq, width, self.chunk.score_dtype, dev),
+                    path=_merged(nq, width, self.path.score_dtype, dev))
+
+    def fuse(self, q_ptr, q_terms, path_q_ptr, path_q_terms, k_chunk: int = 192, k_path: int = 6, k_out: int = 256,
+             q_group=None):
+        """Same arguments and result as ``batched.dual_sparse_fusion`` (the term lists of each index's vocabulary);
+        ``k_chunk`` and ``k_path`` in [1, 1024]."""
+        from . import batched
+        _check_depth("k_chunk", k_chunk)
+        _check_depth("k_path", k_path)
+        if k_out < 1:
+            raise ValueError(f"k_out={k_out} must be >= 1")
+        nq = q_ptr.numel() - 1
+        if path_q_ptr.numel() - 1 != nq:
+            raise ValueError(f"{nq} chunk queries but {path_q_ptr.numel() - 1} path queries")
+        key = (nq, k_chunk, k_path)
+        if key not in self._state:
+            self._state[key] = self._make(nq, k_chunk, k_path)
+        st = self._state[key]
+        batched.bm25_topk(self.chunk, q_ptr, q_terms, k_chunk, q_group=q_group, ws=self.ws, out=st["c_local"])
+        batched.bm25_topk(self.path, path_q_ptr, path_q_terms, k_path, q_group=q_group, ws=self.ws, out=st["p_local"])
+        dist.all_gather_into_tensor(st["gathered"], st["record"], group=self.group)   # the one collective
+        g_cs, g_ci, g_ps, g_pi = st["views"]
+        a = batched.merge_sorted_parts(g_cs, g_ci, self.world, st["nbytes"], k_chunk, out=st["chunk"])
+        b = batched.merge_sorted_parts(g_ps, g_pi, self.world, st["nbytes"], k_path, out=st["path"])
+        return batched.fusion_simple(a.ids, a.scores, a.counts, b.ids, b.scores, b.counts, k_out, canon=self.canon)
 
 
 def token_balanced_ranges(cu_h: Sequence[int], world: int) -> List[Tuple[int, int]]:

@@ -196,6 +196,15 @@ int ezr_merge_topk_parts(const void* cand_scores, const int32_t* cand_ids, int32
                          int32_t n_cand, int64_t cand_stride, int32_t n_parts, int64_t part_stride_bytes, int32_t k,
                          void* out_scores, int32_t* out_ids, int32_t* out_counts, void* stream);
 
+/* Merge of SORTED per-shard lists, k <= 1024 (csrc/merge.cu).  n_parts lists per row, read in place from the gathered
+ * records (addressing as ezr_merge_topk_parts).  Each part's slots are in canonical order (score desc, id desc) up to
+ * its first id < 0, and hold only ids < 0 after it; ids are distinct across parts (disjoint shards).  Output: the
+ * canonical top-k of the union at row q * out_stride, counts = min(k, total valid); slots [count, out_stride) get
+ * id -1 and score -inf.  k, n_cand <= 1024, n_parts * n_cand <= 8192, out_stride >= k. */
+int ezr_merge_sorted_parts(const void* cand_scores, const int32_t* cand_ids, int32_t score_type, int32_t n_rows,
+                           int32_t n_cand, int64_t cand_stride, int32_t n_parts, int64_t part_stride_bytes, int32_t k,
+                           void* out_scores, int32_t* out_ids, int32_t* out_counts, int64_t out_stride, void* stream);
+
 /* ------------------------------------------------------------- dense ----
  * QdrantRetriever (retrievers.py:37-52) over a COSINE collection (ingestion.py:180-182):
  * corpus rows and queries are L2-normalised bf16; score = fp32-accumulated dot product.
