@@ -1,5 +1,5 @@
-// Entry points of the wgmma attention kernel (attention_tc.cuh): argument checks, tensor maps, the plan buffer and the
-// bidirectional instances.  ezr_attn_set_kernel(1) routes ezr_attn_bidir to the warp-level mma.sync kernel
+// Entry points of the wgmma attention kernel (attention_tc.cuh): argument checks, tensor maps and the bidirectional
+// instances.  ezr_attn_set_kernel(1) routes ezr_attn_bidir to the warp-level mma.sync kernel
 // (attention.cu) instead.
 #include "attention_tc.cuh"
 
@@ -12,28 +12,6 @@ int attn_bidir_legacy(const void* qkv, int64_t ld, const int32_t* cu_seqlens, in
 static int g_attn_kernel = 0;     // ezr_attn_set_kernel: 0 = wgmma (default), 1 = legacy mma.sync kernel (cross-checks,
                                   // bidirectional only)
 static thread_local const char* g_attn_last = "none";
-
-// plan buffer (query-block list) of the calling thread's device, grown on demand
-static thread_local int32_t* g_plan = nullptr;
-static thread_local size_t g_plan_cap = 0;
-static thread_local int g_plan_dev = -1;
-
-int attn_plan_buffer(size_t n_items, int4** plan, int32_t** plan_n) {
-    const size_t need = (n_items + 1) * 4;          // ints: 4 for the count (keeps the entries 16-byte aligned) + 4 per entry
-    int dev = 0;
-    EZR_CUDA(cudaGetDevice(&dev));
-    if (need > g_plan_cap || dev != g_plan_dev) {         // first call / larger batch / other device: (re)allocate
-        if (g_plan && dev == g_plan_dev) EZR_CUDA(cudaFree(g_plan));
-        g_plan_dev = dev;
-        g_plan = nullptr;
-        g_plan_cap = 0;
-        EZR_CUDA(cudaMalloc(&g_plan, need * 2 * sizeof(int32_t)));
-        g_plan_cap = need * 2;
-    }
-    *plan_n = g_plan;
-    *plan = reinterpret_cast<int4*>(g_plan + 4);
-    return EZR_OK;
-}
 
 // the entry points' shared argument checks and dispatch
 static int attn_run(bool causal, const void* qkv, int64_t n_tokens, int64_t ld, const int32_t* cu_seqlens, int32_t n_seq,

@@ -307,10 +307,9 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
     }
 }
 
-// plan buffer of the calling thread's device with room for n_items entries (attention_tc.cu)
-int attn_plan_buffer(size_t n_items, int4** plan, int32_t** plan_n);
-
-// plan + attention kernel on the caller's tensor maps (scale_log2 = softmax scale * log2 e)
+// plan + attention kernel on the caller's tensor maps (scale_log2 = softmax scale * log2 e).  The plan of a call is
+// its own: drawn from the stream-ordered pool of the launch stream before the plan kernel and released after the
+// attention kernel, so calls on different streams never share it, and graph capture records both as memory nodes.
 template <int HD, bool CAUSAL>
 static int attn_tc_launch(const CUtensorMap& map_q, const CUtensorMap& map_kv, const int32_t* cu, int n_seq, int max_len,
                           int n_heads, int n_kv_heads, float scale_log2, __nv_bfloat16* out, int64_t ldo, cudaStream_t st) {
@@ -321,18 +320,28 @@ static int attn_tc_launch(const CUtensorMap& map_q, const CUtensorMap& map_kv, c
         attr_done = true;
     }
     const int max_qb = (max_len + AT_M - 1) / AT_M;
-    int32_t* plan_n = nullptr;
-    int4* plan = nullptr;
-    const int rc = attn_plan_buffer((size_t)n_seq * max_qb, &plan, &plan_n);
-    if (rc) return rc;
+    const size_t n_items = (size_t)n_seq * max_qb;              // query blocks at most
+    // ints: 4 for the count (keeps the entries 16-byte aligned) + 4 per entry
+    int32_t* buf = nullptr;
+    EZR_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), (n_items + 1) * 4 * sizeof(int32_t), st));
+    int32_t* plan_n = buf;
+    int4* plan = reinterpret_cast<int4*>(buf + 4);
     ProfScope prof(EZR_PROF_ENC_ATTN, st);
     attn_plan_kernel<CAUSAL><<<1, 256, 0, st>>>(cu, n_seq, plan, plan_n);
-    EZR_LAUNCH_CHECK();
-    long long upper = (long long)n_seq * max_qb * n_heads;      // work items at most
-    if (CAUSAL) upper = (upper + 1) / 2;                        // causal CTAs take items in pairs
-    const int grid = (int)(upper < sm_count() ? upper : sm_count());
-    attn_wgmma_kernel<HD, CAUSAL><<<grid, AT_THREADS, smem, st>>>(map_q, map_kv, plan, plan_n, n_heads, n_kv_heads, scale_log2, out, ldo);
-    EZR_LAUNCH_CHECK();
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        long long upper = (long long)n_items * n_heads;         // work items at most
+        if (CAUSAL) upper = (upper + 1) / 2;                    // causal CTAs take items in pairs
+        const int grid = (int)(upper < sm_count() ? upper : sm_count());
+        attn_wgmma_kernel<HD, CAUSAL><<<grid, AT_THREADS, smem, st>>>(map_q, map_kv, plan, plan_n, n_heads, n_kv_heads,
+                                                                      scale_log2, out, ldo);
+        count_launch();
+        e = cudaGetLastError();
+    }
+    const cudaError_t e_free = cudaFreeAsync(buf, st);          // released on every path, after the last reader
+    EZR_CUDA(e);
+    EZR_CUDA(e_free);
     return EZR_OK;
 }
 

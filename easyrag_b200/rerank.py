@@ -29,7 +29,7 @@ from .schema import BaseNodePostprocessor, Field, MetadataMode, NodeWithScore, P
 DEFAULT_SENTENCE_TRANSFORMER_MAX_LENGTH = 512
 DEFAULT_MAX_TOKENS = 65536
 MAX_CANDIDATES = 1024          # candidates per query the ordering kernel holds (one CTA per query)
-MAX_CHUNK_PAIRS = 65535        # sequences one attention launch takes (its grid's y extent)
+MAX_CHUNK_PAIRS = 65535        # sequences one attention call takes (ezr_attn_bidir refuses more, for either kernel)
 
 # family -> (separators between the two segments, token type of the second segment); see ezr_cross_pack_plan
 _TEMPLATES = {"bert": (1, 1), "roberta": (2, 0)}

@@ -14,8 +14,12 @@
  *   - all pointers are DEVICE pointers unless the name ends in _host.
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
  *   - launch functions never allocate: outputs and the workspace are caller-owned
- *     (query the size with the *_workspace call).  They do not synchronise, except
- *     where a function says so (ezr_dense_s8_topk, the rerank packers below).
+ *     (query the size with the *_workspace call).  The one exception is the
+ *     attention entry points (ezr_attn_bidir / ezr_attn_causal), which draw their
+ *     small per-call plan from the stream-ordered memory pool of the launch stream
+ *     (cudaMallocAsync / cudaFreeAsync: no device-wide wait, graph-capturable).
+ *     They do not synchronise, except where a function says so
+ *     (ezr_dense_s8_topk, the rerank packers below).
  *   - document ids are int32, local to the shard the index was built over;
  *     `id_base` is added on output so a row-sharded corpus yields global ids.
  *   - canonical rank order everywhere: score descending, then id descending
@@ -401,7 +405,10 @@ int ezr_layernorm_fp8(const void* x, int64_t ldx, const void* gamma, const void*
                       void* stream);
 /* non-causal attention over packed q|k|v rows ([n_tokens, (H + 2*KV) * hd], row stride ld); head_dim 64 or 128; GQA
  * via n_kv_heads.  Default kernel: wgmma (S = QK^T and O += PV on the tensor cores, S/P/O in registers,
- * Q/K/V tiles by TMA).  n_tokens bounds the TMA tensor map (tiles that run past the last token are zero-filled). */
+ * Q/K/V tiles by TMA).  n_tokens bounds the TMA tensor map (tiles that run past the last token are zero-filled).
+ * n_seq <= 65535 per call (both kernels).  The wgmma kernel's query-block plan (16 bytes per 128-row block) is
+ * allocated on `stream` from its device's default memory pool and freed on it after the kernel, so calls on
+ * different streams, from any thread, never share one; the call can be captured into a CUDA graph. */
 int ezr_attn_bidir(const void* qkv, int64_t n_tokens, int64_t ld, const int32_t* cu_seqlens, int32_t n_seq,
                    int32_t max_len, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, float softmax_scale, void* out,
                    int64_t ldo, void* stream);

@@ -65,7 +65,7 @@ def run_case(lens, H, KV, hd, rounds: int) -> dict:
     out_c = torch.empty_like(out_b)
     f_b = lambda: enc.attention(qkv, cu, max(lens), H, KV, hd, out=out_b)
     f_c = lambda: enc.attention(qkv, cu, max(lens), H, KV, hd, out=out_c, causal=True)
-    for f in (f_b, f_c):                                       # warm-up: module load, function attributes, plan buffer
+    for f in (f_b, f_c):                                       # warm-up: module load, function attributes, the plan pool
         f()
     torch.cuda.synchronize()
     assert _lib.lib().ezr_attn_last_kernel() == b"wgmma-causal"

@@ -18,7 +18,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from _bounds import U32, rejects, round_bf16, ulp_bf16
+from _attn_ref import _causal_check as _check, _causal_ref as _ref, _kernel_tiles
+from _bounds import rejects
 from _oracle_causal import gte_embed_causal, load_golden
 from oracle import encoder as oenc
 from easyrag_b200 import _lib, encoder as enc
@@ -26,7 +27,6 @@ from easyrag_b200.encoder import PackedBatch, Qwen2Config, Qwen2Encoder, random_
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-LAM = 4.0              # probabilistic accumulation bound, as in test_gpu_model_shapes.py
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -54,76 +54,6 @@ def _bidir(qkv, lens, H, KV, hd):
     out = enc.attention(qkv, _cu(lens), max(lens), H, KV, hd)
     torch.cuda.synchronize()
     return out
-
-
-# ------------------------------------------------------------------------------------------ fp64 reference
-def _ref(rows, H, KV, hd, scale, hi):
-    """fp64 attention of one sequence ([n, (H + 2 KV) hd] bf16 rows) where query row r sees keys 0 .. hi[r] - 1.
-    -> (out, p_absv, emu, eps_p), each [n, H, *]: out = softmax(q k^T scale) v over the visible keys; p_absv the same
-    applied to |v|; emu the kernel's rounding points in fp64 (P rounded to bf16 for the numerator, the row sum of the
-    unrounded P, output rounded to bf16); eps_p a bound on the relative error of each kernel P value."""
-    n = rows.shape[0]
-    kvi = torch.tensor([h // (H // KV) for h in range(H)], device=DEV)
-    r = rows.double()
-    q = r[:, :H * hd].view(n, H, hd).transpose(0, 1)
-    k = r[:, H * hd:(H + KV) * hd].view(n, KV, hd).index_select(1, kvi).transpose(0, 1)
-    v = r[:, (H + KV) * hd:(H + 2 * KV) * hd].view(n, KV, hd).index_select(1, kvi).transpose(0, 1)
-    hi = torch.as_tensor(hi, device=DEV)
-    o, pa, em = (torch.empty(H, n, hd, dtype=torch.float64, device=DEV) for _ in range(3))
-    ep = torch.empty(H, n, 1, dtype=torch.float64, device=DEV)
-    step = max(1, (1 << 25) // (H * n))
-    cols = torch.arange(n, device=DEV)
-    for c0 in range(0, n, step):
-        vis = (cols[None, :] < hi[c0:c0 + step, None])[None]            # [1, rows, n]
-        qc = q[:, c0:c0 + step]
-        s = (qc @ k.transpose(1, 2)).masked_fill(~vis, -math.inf)
-        m = s.amax(-1, keepdim=True)
-        p = torch.exp((s - m) * scale)
-        l = p.sum(-1, keepdim=True)
-        o[:, c0:c0 + step] = (p @ v) / l
-        pa[:, c0:c0 + step] = (p @ v.abs()) / l
-        em[:, c0:c0 + step] = round_bf16((round_bf16(p) @ v) / l)
-        qk = (qc.abs() @ k.abs().transpose(1, 2)).masked_fill(~vis, 0).amax(-1, keepdim=True)
-        sa = s.abs().masked_fill(~vis, 0).amax(-1, keepdim=True)
-        ep[:, c0:c0 + step] = (scale * LAM * math.sqrt(hd) * U32 * qk    # fp32 accumulation of the logits
-                               + 3 * U32 * scale * (sa + m.abs())        # fma(s, scale log2 e, -m scale log2 e)
-                               + 2.0 ** -22)                             # ex2.approx.ftz (2 ulp)
-        del s, p
-    return tuple(t.transpose(0, 1) for t in (o, pa, em, ep))
-
-
-def _kernel_tiles(n):
-    """Key tiles the kernel walks for each row's 128-row item: min(ceil(n / 64), q0 / 64 + 2)."""
-    r = torch.arange(n, device=DEV)
-    return torch.clamp((r // 128) * 2 + 2, max=(n + 63) // 64).double()
-
-
-def _check(got, ref, keys, tiles, what):
-    """got [n, H, hd] bf16 against a reference: per-element bound (row r accumulates keys[r] terms over tiles[r] key
-    tiles) and per-head rms error at most 1.5 x that of the fp64 emulation.  Returns the worst rms ratio."""
-    o, pa, em, ep = ref
-    g = got.double()
-    keys = keys.double()[:, None, None]
-    tiles = tiles[:, None, None]
-    main = 2.0 ** -8 * pa                          # P rounded to bf16 before P V (relative 2^-9 per term, doubled)
-    bound = (main
-             + (2 * ep                             # the P values' own error, in the numerator and in the row sum
-                + (2 * tiles                       # O and the row sum rescaled by alpha once per key tile (fp32)
-                   + LAM * keys.sqrt()             # fp32 accumulation of P V over the visible keys
-                   + 2) * U32)                     # 1 / l and O * (1 / l)
-             * (pa + o.abs())
-             + ulp_bf16(o.abs() + main))           # the bf16 output rounding
-    err = (g - o).abs()
-    worst = int(torch.argmax(err / bound))
-    assert (err <= bound).all(), (f"{what}: worst element {worst}: |err| {err.reshape(-1)[worst].item():.3g} vs bound "
-                                  f"{bound.reshape(-1)[worst].item():.3g}")
-    den = o.pow(2).sum((0, 2)).sqrt().clamp_min(1e-300)
-    e_got = (g - o).pow(2).sum((0, 2)).sqrt() / den
-    e_emu = (em - o).pow(2).sum((0, 2)).sqrt() / den
-    bad = e_got > 1.5 * e_emu + 1e-12
-    assert not bad.any(), (f"{what}: rms error of heads {torch.nonzero(bad).flatten().tolist()}: "
-                           f"{e_got[bad].tolist()} vs emulation {e_emu[bad].tolist()}")
-    return torch.where(e_emu > 0, e_got / e_emu.clamp_min(1e-300), torch.zeros_like(e_got)).max().item()
 
 
 LENS = [1, 2, 63, 64, 65, 127, 128, 129, 300, 1024, 4097, 8192]

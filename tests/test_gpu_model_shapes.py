@@ -15,6 +15,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from _attn_ref import _attn_check, _attn_ref
 from _bounds import U32, check_bf16, ln_exact_and_delta, rejects, round_bf16, ulp_bf16
 from _topk_ref import canonical_topk
 from oracle import encoder as oenc
@@ -313,76 +314,6 @@ def test_pool_mean_8192_and_1_token(l2):
 
 
 # -------------------------------------------------------------------------------------------- attention
-def _attn_ref(qkv, lens, H, KV, hd, scale, seqs=None, kv_of_head=None, drop=None):
-    """fp64 attention per (sequence, head) with query rows chunked.  Returns {seq: (out, p_absv, emu, eps_p)}:
-    out = softmax(q k^T scale) v; p_absv = the same applied to |v|; emu = the kernel's rounding points emulated in fp64
-    (P rounded to bf16 for the numerator, the row sum of unrounded P, output rounded to bf16); eps_p = a bound on the
-    relative error of each kernel P value.  ``kv_of_head`` / ``drop`` (a key range of one sequence) build controls."""
-    kv_of_head = kv_of_head if kv_of_head is not None else [h // (H // KV) for h in range(H)]
-    kvi = torch.tensor(kv_of_head, device=DEV)
-    cu = np.cumsum([0] + list(lens))
-    out = {}
-    for b in (seqs if seqs is not None else range(len(lens))):
-        lo, n = int(cu[b]), int(lens[b])
-        rows = qkv[lo:lo + n].double()
-        q = rows[:, :H * hd].view(n, H, hd).transpose(0, 1)
-        k = rows[:, H * hd:(H + KV) * hd].view(n, KV, hd).index_select(1, kvi).transpose(0, 1)
-        v = rows[:, (H + KV) * hd:(H + 2 * KV) * hd].view(n, KV, hd).index_select(1, kvi).transpose(0, 1)
-        if drop is not None and drop[0] == b:
-            keep = torch.ones(n, dtype=torch.bool, device=DEV)
-            keep[drop[1]:drop[2]] = False
-            k, v = k[:, keep], v[:, keep]
-        o, pa, em = (torch.empty(H, n, hd, dtype=torch.float64, device=DEV) for _ in range(3))
-        ep = torch.empty(H, n, 1, dtype=torch.float64, device=DEV)
-        step = max(1, (1 << 25) // (H * k.shape[1]))
-        for c0 in range(0, n, step):
-            qc = q[:, c0:c0 + step]
-            s = qc @ k.transpose(1, 2)
-            m = s.amax(-1, keepdim=True)
-            p = torch.exp((s - m) * scale)
-            l = p.sum(-1, keepdim=True)
-            o[:, c0:c0 + step] = (p @ v) / l
-            pa[:, c0:c0 + step] = (p @ v.abs()) / l
-            em[:, c0:c0 + step] = round_bf16((round_bf16(p) @ v) / l)
-            qk = (qc.abs() @ k.abs().transpose(1, 2)).amax(-1, keepdim=True)
-            ep[:, c0:c0 + step] = (scale * LAM * math.sqrt(hd) * U32 * qk     # fp32 accumulation of the logits
-                                   + 3 * U32 * scale * (s.abs().amax(-1, keepdim=True) + m.abs())
-                                   # fma(s, scale log2 e, -m scale log2 e) and its rounded operands
-                                   + 2.0 ** -22)                               # ex2.approx.ftz (2 ulp)
-            del s, p
-        out[b] = (o.transpose(0, 1), pa.transpose(0, 1), em.transpose(0, 1), ep.transpose(0, 1))
-    return out
-
-
-def _attn_check(got, ref, n, what):
-    """got [n, H, hd] (bf16) against one sequence's reference: a per-element bound and a per-head rms ratio.
-    Returns the worst rms ratio (kernel error / emulated error)."""
-    o, pa, em, ep = ref
-    g = got.double()
-    n_tiles = (n + 63) // 64
-    main = 2.0 ** -8 * pa                          # P rounded to bf16 before P V (relative 2^-9 per term, doubled)
-    bound = (main
-             + (2 * ep                             # the P values' own error, in the numerator and in the row sum
-                + (2 * n_tiles                     # O and the row sum rescaled by alpha once per key tile (fp32)
-                   + LAM * math.sqrt(n)            # fp32 accumulation of P V over the keys
-                   + 2) * U32)                     # 1 / l and O * (1 / l)
-             * (pa + o.abs())
-             + ulp_bf16(o.abs() + main))           # the bf16 output rounding
-    err = (g - o).abs()
-    worst = int(torch.argmax(err / bound))
-    assert (err <= bound).all(), (f"{what}: worst element {worst}: |err| {err.reshape(-1)[worst].item():.3g} vs bound "
-                                  f"{bound.reshape(-1)[worst].item():.3g}")
-    # per head: relative rms error vs fp64 <= 1.5 x that of the fp64 emulation of the kernel's rounding points
-    den = o.pow(2).sum((0, 2)).sqrt().clamp_min(1e-300)
-    e_got = (g - o).pow(2).sum((0, 2)).sqrt() / den
-    e_emu = (em - o).pow(2).sum((0, 2)).sqrt() / den
-    ratio = e_got / e_emu.clamp_min(1e-300)
-    bad = e_got > 1.5 * e_emu + 1e-12
-    assert not bad.any(), (f"{what}: rms error of heads {torch.nonzero(bad).flatten().tolist()}: "
-                           f"{e_got[bad].tolist()} vs emulation {e_emu[bad].tolist()}")
-    return torch.where(e_emu > 0, ratio, torch.zeros_like(ratio)).max().item()
-
-
 ATTN_CASES = [  # (H, KV, hd, lengths)
     (28, 4, 128, [1, 8, 48, 129, 4097, 300, 1024, 8192]),      # gte-Qwen2-7B: GQA group 7; 8192 ends the buffer
     (16, 16, 64, [512, 1, 77, 256, 129, 500, 64, 3, 511]),     # XLM-R-large cross-encoder
