@@ -55,7 +55,10 @@ def qwen2_hidden_causal(state: Dict[str, torch.Tensor], cfg, input_ids: torch.Te
         k = k.repeat_interleave(H // KV, dim=1)
         v = v.repeat_interleave(H // KV, dim=1)
         att = torch.matmul(q, k.transpose(2, 3)) / math.sqrt(hd) + add
-        att = F.softmax(att, dim=-1, dtype=torch.float32).to(dtype)
+        # the reference's softmax runs in float32; a float64 evaluation keeps float64, where float64's minimum stays
+        # finite.  Cast to float32 it is -inf, a padding query row (which sees no real key) turns NaN, and 0 * NaN
+        # carries that into every real row of the next layer through the padding keys and values.
+        att = F.softmax(att, dim=-1, dtype=torch.float64 if dtype == torch.float64 else torch.float32).to(dtype)
         o = torch.matmul(att, v).transpose(1, 2).reshape(b, l, H * hd)
         x = res + F.linear(o, w[p + "self_attn.o_proj.weight"])
         res = x

@@ -28,6 +28,17 @@ def test_causal_oracle_bf16_tracks_reference_bf16():
     assert cos.min() > 1 - 1e-3
 
 
+def test_causal_oracle_fp64_on_left_padded_batches():
+    # the float64 evaluation the GPU tests compare against: every sequence but the longest is left-padded, so padding
+    # query rows see no real key.  With the softmax in float32 the float64 mask became -inf there and NaN reached every
+    # padded sequence's embedding through the second layer.
+    z, cfg, state = load_golden()
+    assert cfg.num_hidden_layers >= 2 and (z["attention_mask"][:, 0] == 0).sum() >= 2
+    got = gte_embed_causal(state, cfg, *_inputs(z), torch.float64).numpy()
+    assert np.isfinite(got).all()
+    assert np.abs(got - z["emb_fp32"]).max() < 2e-6
+
+
 def test_causal_golden_differs_from_bidirectional_oracle():
     # the same weights through the bidirectional oracle land far from the causal reference: the file pins the mask
     z, cfg, state = load_golden()
