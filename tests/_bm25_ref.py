@@ -42,6 +42,15 @@ def counts(tokens, doc_ptr, vocab, doc_lo=0, doc_hi=None):
                 first_pos=first, doc_len=lens.to(torch.int64))
 
 
+def postings_of_docs(indptr, post_doc, doc_lo, doc_hi):
+    """The postings of documents ``[doc_lo, doc_hi)`` picked out of a whole term-major index (``indptr`` int64 [V+1],
+    ``post_doc`` int [P], one device), in the index's order: -> dict(pos, term, doc) int64, ``pos`` the index of each
+    posting in the whole arrays.  What :func:`counts` of the same documents lists, and what a row shard holds."""
+    pos = torch.nonzero((post_doc >= doc_lo) & (post_doc < doc_hi)).flatten()
+    term = torch.searchsorted(indptr[1:], pos, right=True)
+    return dict(pos=pos, term=term, doc=post_doc[pos].to(torch.int64))
+
+
 def _t(x, like):
     """A 0-dim float64 tensor on ``like``'s device (a tensor divisor keeps the division IEEE on CUDA)."""
     return torch.tensor(float(x), dtype=torch.float64, device=like.device)

@@ -20,17 +20,23 @@ def _lib():
     return _lib
 
 
-def rescore_all(q: torch.Tensor, c: torch.Tensor, q_chunk: int = 64) -> torch.Tensor:
-    """[Q, N] float32 rescore values (``-0.0`` as ``+0.0``)."""
-    ct = c.float().T.contiguous()                       # [dim, N]
+def rescore_all(q: torch.Tensor, c: torch.Tensor, q_chunk: int = 64, row_chunk: int = 0) -> torch.Tensor:
+    """[Q, N] float32 rescore values (``-0.0`` as ``+0.0``).  ``row_chunk`` > 0 converts the corpus to float32 that
+    many rows at a time (the same operations per element, so the same bits; a 4M x 1024 float copy would be 16 GB)."""
+    n = c.shape[0]
+    row_chunk = row_chunk if row_chunk > 0 else max(n, 1)
     qf = q.float()
-    out = torch.empty(q.shape[0], c.shape[0], dtype=torch.float32, device=q.device)
-    for q0 in range(0, q.shape[0], q_chunk):
-        qq = qf[q0:q0 + q_chunk]
-        acc = torch.zeros(qq.shape[0], c.shape[0], dtype=torch.float32, device=q.device)
-        for i in range(c.shape[1]):
-            acc = acc + qq[:, i:i + 1] * ct[i][None, :]
-        out[q0:q0 + q_chunk] = acc + 0.0
+    out = torch.empty(q.shape[0], n, dtype=torch.float32, device=q.device)
+    for r0 in range(0, n, row_chunk):
+        r1 = min(n, r0 + row_chunk)
+        ct = c[r0:r1].float().T.contiguous()            # [dim, rows]
+        for q0 in range(0, q.shape[0], q_chunk):
+            qq = qf[q0:q0 + q_chunk]
+            acc = torch.zeros(qq.shape[0], r1 - r0, dtype=torch.float32, device=q.device)
+            for i in range(c.shape[1]):
+                acc = acc + qq[:, i:i + 1] * ct[i][None, :]
+            out[q0:q0 + q_chunk, r0:r1] = acc + 0.0
+        del ct
     return out
 
 
