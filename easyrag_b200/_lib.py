@@ -79,6 +79,10 @@ SIGNATURES = {
     "ezr_dense_s8_topk": (C.c_int, [_p, _i64, _i32, _i64, _p, _i32, _i64, _i32, _p, _p, _i32, _p, _p, _p, _p, _i64,
                                     _p, _p, _p, _p, _sz, _p]),
     "ezr_dense_s8_set_capacity": (C.c_int, [_i32]),
+    "ezr_dense_cand_topk_workspace": (_sz, [_i64, _i32, _i32, _i32]),
+    "ezr_dense_cand_topk": (C.c_int, [_p, _i64, _i32, _i64, _p, _i32, _i64, _i32, _p, _p, _i32, _p, _p, _p, _p, _p,
+                                      _sz, _p]),
+    "ezr_dense_cand_set_capacity": (C.c_int, [_i32]),
     "ezr_dense_set_kernel": (C.c_int, [_i32]),
     "ezr_dense_last_kernel": (C.c_char_p, []),
     "ezr_dense_wide_workspace": (_sz, [_i64, _i32, _i32, _i32]),
@@ -187,7 +191,7 @@ PROF_SLOTS = {"bm25_cand": 8, "bm25_rescore": 9,
               "bm25_score": 0, "dense_tc": 1, "dense_simt": 2, "merge": 3, "fuse": 4,
               "enc_gemm": 5, "enc_attn": 6, "enc_other": 7,
               "dense_s8_scan": 10, "dense_s8_rescore": 11, "dense_s8_full": 12, "dense_wide": 13,
-              "bm25_bound": 14}
+              "bm25_bound": 14, "dense_cand_gemm": 15, "dense_cand_bound": 16}
 
 
 def profile_read(name: str):

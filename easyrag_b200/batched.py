@@ -117,6 +117,46 @@ def _dense_topk(index, queries, k, q_group, id_base, ws, stream, out, cand_count
     return out
 
 
+def dense_topk_cand(index: DenseIndex, queries: torch.Tensor, k: int, q_group: Optional[torch.Tensor] = None,
+                    id_base: Optional[int] = None, ws: Optional[Workspace] = None, stream=None,
+                    out: Optional[TopK] = None, cand_counts: Optional[torch.Tensor] = None) -> TopK:
+    """Cosine top-k of the bf16 rows without score rows (``ezr_dense_cand_topk``, csrc/dense_cand.cu): the canonical
+    top-k under form 6's scores, bit-identical to ``dense_topk(..., form=6)``, for any dim % 64 == 0 and k <= 1024.
+
+    Its workspace grows with Q * (k + capacity) where form 6's grows with Q * n_rows, and the whole batch shares one
+    pass over the corpus.  ``cand_counts`` (int32 [Q] on the device) receives the candidates each query emitted, or -1
+    for a query whose buffer overflowed and that form 6 answered inside the call.  A quantized index is searched on
+    its bf16 rows."""
+    L = _lib.lib()
+    dev = index.device
+    q = queries
+    if q.dtype != torch.bfloat16 or q.device != dev or not q.is_contiguous():
+        q = queries.to(device=dev, dtype=torch.bfloat16).contiguous()
+    nq, dim = q.shape
+    if dim != index.dim:
+        raise ValueError(f"query dim {dim} != corpus dim {index.dim}")
+    qg = _i32(q_group, dev)
+    if qg is not None and index.doc_group is None:
+        raise ValueError("q_group given but the index has no doc_group")
+    if cand_counts is not None and (cand_counts.dtype != torch.int32 or cand_counts.numel() < nq
+                                    or cand_counts.device != q.device or not cand_counts.is_contiguous()):
+        raise ValueError("cand_counts must be an int32 device tensor with one slot per query")
+    if out is None:
+        out = TopK(torch.empty(nq, k, dtype=torch.float32, device=dev), torch.empty(nq, k, dtype=torch.int32, device=dev),
+                   torch.empty(nq, dtype=torch.int32, device=dev))
+    need = L.ezr_dense_cand_topk_workspace(index.n_rows, dim, nq, k)
+    ws = ws or Workspace(dev)
+    buf = ws.get(need)
+    base = index.row_lo if id_base is None else id_base
+    with torch.cuda.device(dev):
+        _lib.check(L.ezr_dense_cand_topk(
+            _lib.ptr(index.vectors), index.n_rows, dim, index.vectors.stride(0), _lib.ptr(q), nq, q.stride(0), k,
+            _lib.ptr(index.doc_group if qg is not None else None), _lib.ptr(qg), base, _lib.ptr(out.scores),
+            _lib.ptr(out.ids), _lib.ptr(out.counts), _lib.ptr(cand_counts), _lib.ptr(buf), buf.numel(),
+            _lib.stream_ptr(stream)), "ezr_dense_cand_topk")
+    return out
+
+
 def bm25_topk(index: Bm25Index, q_ptr: torch.Tensor, q_terms: torch.Tensor, k: int,
               q_group: Optional[torch.Tensor] = None, id_base: Optional[int] = None,
               ws: Optional[Workspace] = None, stream=None, out: Optional[TopK] = None) -> TopK:

@@ -7,11 +7,9 @@
 // cuBLAS calls behind the reference's projections: Qwen2 q/k/v/o and SwiGLU MLP (modeling_qwen.py:261-263,
 // 319,186) and the BERT-shaped encoder's dense layers behind SentenceTransformer.encode (hf_embeddings.py:118-123).
 //
-// One CTA computes one 128 x 256 output tile.  Warpgroup 0 is the TMA producer (one thread; a 4-stage ring of 128 x 64
-// A tiles and 256 x 64 W tiles, 48 KB a stage); warpgroups 1 and 2 each own 64 rows of the tile and issue
-// wgmma.m64n256k16 from the ring into 128 fp32 accumulator registers per thread, keeping one k-chunk of MMAs in flight
-// while the previous stage is handed back to the producer.  The epilogue runs on the accumulator registers: bias /
-// GELU / SwiGLU / residual in fp32, bf16 pairs stored straight to global memory.  SwiGLU needs no exchange: the gate
+// One CTA computes one 128 x 256 output tile with the mainloop of gemm_tc.cuh (a 4-stage TMA ring feeding
+// wgmma.m64n256k16 into 128 fp32 accumulator registers per consumer thread).  The epilogue runs on the accumulator
+// registers: bias / GELU / SwiGLU / residual in fp32, bf16 pairs stored straight to global memory.  SwiGLU needs no exchange: the gate
 // column c and its "up" column c + 128 of a 256-column tile sit in the same thread.
 //
 // Tile order: N tiles fastest.  The activations of a 147k-token batch (226 MB at K = 768, 905 MB at K = 3072) do not fit
@@ -20,97 +18,29 @@
 //
 // Dense top-k form 6 (dense_wide.cu) runs the same kernel on A = a block of queries, W = the corpus rows, with the
 // EPI_SCORES epilogue (fp32 score rows, gemm_scores_f32) and M tiles fastest: there the query block (a few MB) fits L2
-// and the corpus does not, so the CTAs in flight cover all query tiles of a few corpus tiles.
+// and the corpus does not, so the CTAs in flight cover all query tiles of a few corpus tiles.  The dense candidate pass
+// (dense_cand.cu) runs the same mainloop in the same tile order with an epilogue that keeps only the scores that can
+// still reach each query's top-k.
 #include <type_traits>
 
 #include "../ezr_common.cuh"
 #include "../ptx.cuh"
 #include "../dense_tc.h"
 #include "gemm_epi.cuh"
+#include "gemm_tc.cuh"
 
 namespace ezr {
-
-constexpr int GM = 128, GN = 256, GK = 64;
-constexpr int G_STAGES = 4;
-constexpr int G_THREADS = 384;                 // producer warpgroup + two consumer warpgroups
-constexpr int G_A_BYTES = GM * GK * 2;         // 16 KB
-constexpr int G_B_BYTES = GN * GK * 2;         // 32 KB
-
-struct GemmParams {
-    int M, N, K;
-    int tiles_m, tiles_n;
-    const __nv_bfloat16* bias;       // [N] or null
-    const __nv_bfloat16* residual;   // [M, ldr] or null
-    int64_t ldr;
-    void* out;                       // [M, ldo] bf16; fp32 for EPI_SCORES
-    int64_t ldo;
-};
-
-struct GemmBarriers {
-    uint64_t full[G_STAGES];
-    uint64_t empty[G_STAGES];
-};
 
 template <int EPI, bool M_FAST>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const GemmParams p) {
-    extern __shared__ __align__(1024) unsigned char smem_dyn[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    unsigned char* smem_a = smem;
-    unsigned char* smem_b = smem + (size_t)G_STAGES * G_A_BYTES;
-    GemmBarriers* bars = reinterpret_cast<GemmBarriers*>(smem_b + (size_t)G_STAGES * G_B_BYTES);
     // N tiles fastest, M tiles for the score rows: see the header
     const int tn = M_FAST ? blockIdx.x / p.tiles_m : blockIdx.x % p.tiles_n;
     const int tm = M_FAST ? blockIdx.x % p.tiles_m : blockIdx.x / p.tiles_n;
-    const int kchunks = p.K / GK;
-    const int wg = threadIdx.x >> 7;
-
-    if (threadIdx.x == 0) {
-        ptx::prefetch_tensormap(&map_a);
-        ptx::prefetch_tensormap(&map_w);
-        for (int i = 0; i < G_STAGES; ++i) { ptx::mbar_init(&bars->full[i], 1); ptx::mbar_init(&bars->empty[i], 2); }
-        ptx::fence_barrier_init();
-    }
-    __syncthreads();
-
-    if (wg == 0) {
-        ptx::regs_dealloc<40>();
-        if (threadIdx.x == 0) {
-            for (int kc = 0; kc < kchunks; ++kc) {
-                const int s = kc % G_STAGES;
-                ptx::mbar_wait(&bars->empty[s], ((uint32_t)(kc / G_STAGES) & 1u) ^ 1u);
-                ptx::mbar_expect_tx(&bars->full[s], (uint32_t)(G_A_BYTES + G_B_BYTES));
-                ptx::tma_load_2d(smem_a + (size_t)s * G_A_BYTES, &map_a, &bars->full[s], kc * GK, tm * GM);
-                ptx::tma_load_2d(smem_b + (size_t)s * G_B_BYTES, &map_w, &bars->full[s], kc * GK, tn * GN);
-            }
-        }
-        return;
-    }
-    ptx::regs_alloc<232>();
-    const int cw = wg - 1;                                   // this warpgroup's 64 rows of the tile
-    const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
     float acc[128];
-#pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    const uint32_t a0 = ptx::smem_u32(smem_a) + (uint32_t)(cw * 64 * 128);
-    const uint32_t b0 = ptx::smem_u32(smem_b);
-    for (int kc = 0; kc < kchunks; ++kc) {
-        const int s = kc % G_STAGES;
-        ptx::mbar_wait(&bars->full[s], (uint32_t)(kc / G_STAGES) & 1u);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int k4 = 0; k4 < GK / 16; ++k4)
-            ptx::wgmma_ss_n256(acc, ptx::make_desc_sw128(a0 + (uint32_t)(s * G_A_BYTES + k4 * 32)),
-                               ptx::make_desc_sw128(b0 + (uint32_t)(s * G_B_BYTES + k4 * 32)), (uint32_t)((kc | k4) != 0));
-        ptx::wgmma_commit();
-        if (kc > 0) {                                        // the previous chunk's MMAs are done: hand its stage back
-            ptx::wgmma_wait<1>();
-            if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&bars->empty[(kc - 1) % G_STAGES]);
-        }
-    }
-    ptx::wgmma_wait<0>();
-    ptx::fence_regs(acc);
-    // (the last stage is never handed back: no later load of this CTA needs it)
+    GemmThread t;
+    if (!gemm_tile_mainloop(&map_a, &map_w, tm, tn, p.K / GK, acc, t)) return;
+    const int cw = t.cw, lane = t.lane, wq = t.wq;
 
     // ---------------- epilogue on the accumulator registers
     typedef typename std::conditional<EPI == EPI_SCORES, float, __nv_bfloat16>::type out_t;
@@ -157,7 +87,7 @@ static int gemm_launch(const __nv_bfloat16* A, int M, int K, int64_t lda, const 
     if (rc) return rc;
     rc = encode_tmap_2d_bf16(&map_w, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, GK, GN);
     if (rc) return rc;
-    const size_t smem = 1024 + (size_t)G_STAGES * (G_A_BYTES + G_B_BYTES) + sizeof(GemmBarriers);
+    const size_t smem = G_SMEM_BYTES;
     typedef void (*kern_t)(const CUtensorMap, const CUtensorMap, const GemmParams);
     static const kern_t table[4] = {gemm_wgmma_kernel<EPI_NONE, false>, gemm_wgmma_kernel<EPI_GELU, false>,
                                     gemm_wgmma_kernel<EPI_SWIGLU, false>, gemm_wgmma_kernel<EPI_SCORES, true>};

@@ -204,7 +204,7 @@ class ShardedCoarseRanker:
         self.ranker.join()
 
     def pipeline_hybrid(self, queries, q_ptr, q_terms, k_dense: int = 288, k_sparse: int = 192, k_out: int = 256,
-                        K: int = 60, q_group=None, canon: Optional[torch.Tensor] = None):
+                        K: int = 60, q_group=None, canon: Optional[torch.Tensor] = None, dense_cand: bool = False):
         """dense top-``k_dense`` + BM25 top-``k_sparse`` + RRF to ``k_out`` at the pipeline's depths (pipeline.py's
         f_topk_1 / f_topk_2 / f_topk), each route k in [1, 1024] -> (fused, sparse, dense), bit-identical to one GPU
         running ``dense_topk(k_dense)`` + ``bm25_topk(k_sparse)`` + ``fuse_lists`` over the whole corpus.
@@ -216,7 +216,10 @@ class ShardedCoarseRanker:
 
         Memory: the gathered buffer holds G * Q * (8 * k_dense + (S + 4) * k_sparse) bytes, S the BM25 score size (8
         for Okapi, 4 for bm25s): 369 MB at G = 8, Q = 10k, 288 / 192, float64.  Batches are not split into query
-        blocks, so a very large Q needs the caller to split it."""
+        blocks, so a very large Q needs the caller to split it.
+
+        ``dense_cand=True`` runs the dense route with ``dense_topk_cand`` (form 6's scores without score rows) on every
+        shard; the result is then bit-identical to one GPU running ``dense_topk_cand`` in place of ``dense_topk``."""
         from . import batched
         _check_depth("k_dense", k_dense)
         _check_depth("k_sparse", k_sparse)
@@ -241,7 +244,10 @@ class ShardedCoarseRanker:
                 fused=_merged(nq, k_out, torch.float64, dev))
         st = self._state[key]
         batched.bm25_topk(r.sparse, q_ptr, q_terms, k_sparse, q_group=q_group, ws=r.ws_sparse, out=st["s_local"])
-        batched.dense_topk(r.dense, queries, k_dense, q_group=q_group, ws=r.ws_dense, out=st["d_local"])
+        if dense_cand:
+            batched.dense_topk_cand(r.dense, queries, k_dense, q_group=q_group, ws=r.ws_dense, out=st["d_local"])
+        else:
+            batched.dense_topk(r.dense, queries, k_dense, q_group=q_group, ws=r.ws_dense, out=st["d_local"])
         dist.all_gather_into_tensor(st["gathered"], st["record"], group=self.group)   # the one collective
         g_ds, g_di, g_ss, g_si = st["views"]
         nbytes = st["layout"].nbytes

@@ -127,16 +127,21 @@ class B200VectorStore:
 
     ``dense_form`` / ``block_queries`` are passed to :func:`easyrag_b200.batched.dense_topk` as ``form`` /
     ``block_queries`` on every query (``dense_form=6``: wgmma score rows, for wide embeddings such as gte-Qwen2-7B's
-    3584 dims or k > 16); the defaults keep the automatic choice.
+    3584 dims or k > 16); the defaults keep the automatic choice.  ``dense_cand=True`` searches with
+    :func:`easyrag_b200.batched.dense_topk_cand` instead (form 6's results without its score rows); it excludes
+    ``dense_form``, ``block_queries`` and ``quantize``.
     """
 
     def __init__(self, nodes: Optional[Sequence[Any]] = None, device="cuda", quantize: bool = False,
-                 dense_form: Optional[int] = None, block_queries: Optional[int] = None):
+                 dense_form: Optional[int] = None, block_queries: Optional[int] = None, dense_cand: bool = False):
+        if dense_cand and (dense_form is not None or block_queries is not None or quantize):
+            raise ValueError("dense_cand=True excludes dense_form, block_queries and quantize")
         if block_queries is not None and (dense_form != 6 or quantize):
             raise ValueError("block_queries needs dense_form=6 and an index that is not quantized")
         self.device = device
         self.dense_form = dense_form
         self.block_queries = block_queries
+        self.dense_cand = bool(dense_cand)
         # keep an int8 mirror: exact search through a certified int8 pass (currently slower than bf16, README)
         self.quantize = bool(quantize)
         self.nodes: List[Any] = []
@@ -181,10 +186,11 @@ class B200VectorStore:
     @classmethod
     def from_embed_model(cls, nodes: Sequence[Any], embed_model, device="cuda", batch_size: Optional[int] = None,
                          quantize: bool = False, dense_form: Optional[int] = None,
-                         block_queries: Optional[int] = None) -> "B200VectorStore":
+                         block_queries: Optional[int] = None, dense_cand: bool = False) -> "B200VectorStore":
         """Corpus encode written in place (replaces pipeline.py:141-158 + ingestion.py:155-191): every batch of
         ``embed_model.embed_tensor`` lands in its slice of the corpus matrix, normalised on the way."""
-        store = cls(device=device, quantize=quantize, dense_form=dense_form, block_queries=block_queries)
+        store = cls(device=device, quantize=quantize, dense_form=dense_form, block_queries=block_queries,
+                    dense_cand=dense_cand)
         nodes = list(nodes)
         bs = int(batch_size or getattr(embed_model, "embed_batch_size", 128) or 128)
         embed_type = getattr(embed_model, "_embed_type", 0)
@@ -223,8 +229,11 @@ class B200VectorStore:
         if doc_group is not None:
             self.index.doc_group = self._doc_group(tuple(conditions.keys()), doc_group)
             q_group = torch.tensor([want], dtype=torch.int32)
-        res = batched.dense_topk(self.index, q, k, q_group=q_group, ws=self._ws, form=self.dense_form,
-                                 block_queries=self.block_queries)
+        if self.dense_cand:
+            res = batched.dense_topk_cand(self.index, q, k, q_group=q_group, ws=self._ws)
+        else:
+            res = batched.dense_topk(self.index, q, k, q_group=q_group, ws=self._ws, form=self.dense_form,
+                                     block_queries=self.block_queries)
         n = int(res.counts[0])
         ids = res.ids[0, :n].tolist()
         sims = res.scores[0, :n].tolist()

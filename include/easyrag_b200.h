@@ -280,6 +280,31 @@ int ezr_dense_s8_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int6
  * emits more is answered by the full scan.  The workspace size depends on it; query the workspace after setting. */
 int ezr_dense_s8_set_capacity(int32_t cap);   /* per host thread */
 
+/* Dense top-k without score rows, "the candidate form" (easyrag_b200/csrc/dense_cand.cu; DESIGN §4.3b).  The arguments,
+ * filters, id_base, padding and canonical order of ezr_dense_topk; the result is the canonical top-k under form 6's
+ * scores (ezr_dense_set_kernel(6)), bit for bit.  The encoder's wgmma GEMM mainloop runs over the corpus in chunks
+ * that double in size, and its epilogue appends to a per-query candidate buffer only the scores at or above the
+ * query's current k-th score; a bound step between chunks keeps the top-k of each buffer and raises that threshold.
+ * Memory grows with n_queries * (k + capacity) instead of n_queries * n_rows, and the whole batch shares one pass
+ * over the corpus.
+ *
+ * A query whose buffer overflows is answered by form 6 inside the call (gathered, scored, scattered back); the call
+ * waits for the candidate pass to learn how many did (one 4-byte copy and one stream synchronisation).
+ * out_cand_counts ([n_queries] or NULL): the candidates each query emitted over the whole call, or -1 for a query
+ * form 6 answered.  dim % 64 == 0, row strides % 8 == 0 and 16-byte aligned rows, else EZR_ERR_UNSUPPORTED (no
+ * silent fall-back to another form); fewer workspace bytes than ezr_dense_cand_topk_workspace: EZR_ERR_WORKSPACE.
+ * n_rows == 0 and n_queries == 0 behave as in ezr_dense_topk. */
+size_t ezr_dense_cand_topk_workspace(int64_t n_rows, int32_t dim, int32_t n_queries, int32_t k);
+int ezr_dense_cand_topk(const void* corpus_bf16, int64_t n_rows, int32_t dim, int64_t ld_corpus,
+                        const void* queries_bf16, int32_t n_queries, int64_t ld_queries, int32_t k,
+                        const int32_t* doc_group, const int32_t* q_group, int32_t id_base, float* out_scores,
+                        int32_t* out_ids, int32_t* out_counts, int32_t* out_cand_counts, void* workspace,
+                        size_t workspace_bytes, void* stream);
+/* Candidate slots per query of ezr_dense_cand_topk (0 = the default, 4k + 1024, as the BM25 deep list; at most 2^20).
+ * Results never depend on it: a query that emits more is answered by form 6.  The workspace size depends on it; query
+ * the workspace after setting. */
+int ezr_dense_cand_set_capacity(int32_t cap);   /* per host thread */
+
 /* ------------------------------------------------------------- fusion ---
  * HybridRetriever.reciprocal_rank_fusion (retrievers.py:256-274): list a first, then list b
  * (the reference passes [sparse, dense], retrievers.py:290); score += 1/(rank+K), rank from 1, fp64;
@@ -470,7 +495,10 @@ typedef enum ezr_prof_slot {
     EZR_PROF_DENSE_S8_FULL = 12,    /* full scan of overflowed queries / k > 16 (gather + score rows + select) */
     EZR_PROF_DENSE_WIDE = 13,       /* gemm_wgmma_kernel's score-row instance (form 6; the select counts as merge) */
     EZR_PROF_BM25_BOUND = 14,       /* bm25_bound_kernel between candidate chunks (also inside EZR_PROF_BM25_CAND) */
-    EZR_PROF_COUNT = 15
+    EZR_PROF_DENSE_CAND_GEMM = 15,  /* dense_cand_kernel (the candidate form's GEMM + threshold epilogue) */
+    EZR_PROF_DENSE_CAND_BOUND = 16, /* dense_cand_init_kernel + dense_cand_bound_kernel (bound steps, outputs); the
+                                     * candidate form's form 6 fallback: EZR_PROF_DENSE_WIDE (+ its select: merge) */
+    EZR_PROF_COUNT = 17
 } ezr_prof_slot;
 /* kernels launched by this library since it was loaded (every launch site counts itself) */
 long long ezr_launch_count(void);
