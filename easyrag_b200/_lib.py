@@ -57,6 +57,7 @@ SIGNATURES = {
     "ezr_bm25_shard_count": (C.c_int, [_p, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
     "ezr_bm25_shard_copy": (C.c_int, [_p, _p, _p, _p, _i32, _i32, _p, _p, _p]),
     "ezr_bm25_pack": (C.c_int, [_p, _p, _i64, _i32, _p, C.POINTER(C.c_int32), _p, _p]),
+    "ezr_bm25_pack_f32": (C.c_int, [_p, _p, _i64, _i32, _p, C.POINTER(C.c_int32), _p, _p]),
     "ezr_bm25_term_max": (C.c_int, [_p, _p, _i32, _p, _p]),
     "ezr_bm25_set_skipping": (C.c_int, [_i32]),
     "ezr_bm25_set_plan": (C.c_int, [_i32]),

@@ -13,12 +13,13 @@
 //    documents); float64 accumulators live in shared memory, query terms are
 //    applied strictly in token order (one barrier per term keeps the float64
 //    sum order of the reference), top-k by threshold -> compact -> rank.  Used
-//    for float32 / negative-idf indices, score rows (k > 32) and as the
-//    hand-over target of the path below.
+//    for indices without packed postings (float32 by default, negative idf),
+//    score rows (k > 32) and as the hand-over target of the path below.
 //  * bm25_cand_kernel + bm25_bound_kernel + bm25_rescore_kernel (bm25_pk.cuh,
-//    "two-phase", the default for the fused top-k): integer upper-bound scores
-//    from 4-byte packed postings with shared-memory atomics, then the exact
-//    ordered float64 score of the surviving candidates only.
+//    "two-phase", the default for the fused top-k of float64 indices, opt-in
+//    for float32 ones): integer upper-bound scores from 4-byte packed postings
+//    with shared-memory atomics, then the exact ordered score (float64 or
+//    float32) of the surviving candidates only.
 // Score vectors never touch HBM on the fused paths.
 #include "ezr_common.cuh"
 #include "select.cuh"
@@ -632,26 +633,28 @@ static int g_bm25_skip = 0;
 static int g_bm25_span = 4;     // ezr_bm25_set_span: ranges in the first candidate launch (then the same again, then doubling)
 static int g_bm25_plan = 1;     // ezr_bm25_set_plan: 1 = per-launch plan table (default), 0 = resolve segments inside the CTAs
 
+// Packed postings (float64 weights from ezr_bm25_pack, float32 ones from ezr_bm25_pack_f32) on a monotone index
 static bool pk_usable(const ezr_bm25_index* ix, int k) {
-    return kPkEnabled && ix->post_pk != nullptr && ix->monotone && ix->score_type == EZR_F64 && k <= 32;
+    return kPkEnabled && ix->post_pk != nullptr && ix->monotone && k <= 32;
 }
 
 // the deep form of the two-phase path (bm25_pk.cuh): the same index types, 32 < k <= kSelMaxK
 static bool pk_deep_usable(const ezr_bm25_index* ix, int k) {
-    return kPkEnabled && ix->post_pk != nullptr && ix->monotone && ix->score_type == EZR_F64 && k > 32 &&
-           k <= kSelMaxK;
+    return kPkEnabled && ix->post_pk != nullptr && ix->monotone && k > 32 && k <= kSelMaxK;
 }
 
 struct PkWorkspace {
     int32_t *thr_key, *thr_q, *cand_cnt, *ovf, *ne_sum, *ovf_n, *ovf_list, *cand_ids, *cand_q, *cand_u;
     uint32_t* ne_mask;
     int2* plan;
-    double* rows;   // deep form: [Q][list_cap] exact scores beside cand_ids
+    void* rows;     // deep form: [Q][list_cap] exact scores (the index's score type) beside cand_ids
     size_t zero_bytes, total;
 };
 
-// list_cap: candidates per query (kPkListCap, or pk_deep_list_cap(k) with deep, which adds the score rows)
-static PkWorkspace pk_carve(void* base, int n_queries, int list_cap = kPkListCap, bool deep = false) {
+// list_cap: candidates per query (kPkListCap, or pk_deep_list_cap(k) with deep, which adds the score rows of
+// score_bytes each)
+static PkWorkspace pk_carve(void* base, int n_queries, int list_cap = kPkListCap, bool deep = false,
+                            size_t score_bytes = 8) {
     PkWorkspace w;
     const size_t q = (size_t)n_queries;
     char* b = reinterpret_cast<char*>(base);
@@ -675,15 +678,17 @@ static PkWorkspace pk_carve(void* base, int n_queries, int list_cap = kPkListCap
     off += align_up(q * lc * 4, 256);
     w.plan = reinterpret_cast<int2*>(b + off);
     off += align_up(q * kPkMaxChunk * kPkPlanTok * sizeof(int2), 256);
-    w.rows = deep ? reinterpret_cast<double*>(b + off) : nullptr;
-    if (deep) off += align_up(q * lc * 8, 256);
+    w.rows = deep ? reinterpret_cast<void*>(b + off) : nullptr;
+    if (deep) off += align_up(q * lc * score_bytes, 256);
     w.total = off;
     return w;
 }
 
-// deep: the deep form's kernels; rescoring then fills w.rows instead of the outputs (the caller selects the top-k)
+// deep: the deep form's kernels; rescoring then fills w.rows instead of the outputs (the caller selects the top-k).
+// S: the index's score type (the kernel instances and their attributes are per type).
+template <typename S>
 static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t* q_terms, int n_queries, int k,
-                     const int32_t* q_group, int id_base, const PkWorkspace& w, double* out_scores,
+                     const int32_t* q_group, int id_base, const PkWorkspace& w, S* out_scores,
                      int32_t* out_ids, int32_t* out_counts, cudaStream_t st, bool deep = false) {
     Bm25Params p;
     p.indptr = ix->indptr; p.post_doc = ix->post_doc; p.post_w = ix->post_w; p.range_off = ix->range_off;
@@ -699,17 +704,17 @@ static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32
     const size_t bd_smem = deep ? pk_deep_bound_smem(k) : 0;
     static bool attr_done = false, deep_attr_done = false;
     if (!deep && !attr_done) {
-        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<false, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<false, S>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                       cudaSharedmemCarveoutMaxShared));
         attr_done = true;
     }
     if (deep && !deep_attr_done) {                      // sized for the largest k
-        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<true, S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)pk_deep_cand_smem(kSelMaxK)));
-        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+        EZR_CUDA(cudaFuncSetAttribute(bm25_cand_kernel<true, S>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                       cudaSharedmemCarveoutMaxShared));
-        EZR_CUDA(cudaFuncSetAttribute(bm25_bound_deep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        EZR_CUDA(cudaFuncSetAttribute(bm25_bound_deep_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)pk_deep_bound_smem(kSelMaxK)));
         deep_attr_done = true;
     }
@@ -729,14 +734,14 @@ static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32
                 bm25_plan_kernel<<<(unsigned)((n_plan + 255) / 256), 256, 0, st>>>(p, r0, len, n_queries, w.plan);
                 EZR_LAUNCH_CHECK();
             }
-            if (deep) bm25_cand_kernel<true><<<dim3(n_queries, len), kPkThreads, smem, st>>>(p, c, r0);
-            else bm25_cand_kernel<false><<<dim3(n_queries, len), kPkThreads, smem, st>>>(p, c, r0);
+            if (deep) bm25_cand_kernel<true, S><<<dim3(n_queries, len), kPkThreads, smem, st>>>(p, c, r0);
+            else bm25_cand_kernel<false, S><<<dim3(n_queries, len), kPkThreads, smem, st>>>(p, c, r0);
             EZR_LAUNCH_CHECK();
             r0 += len;
             if (r0 < ix->n_ranges) {
                 ProfScope prof_bd(EZR_PROF_BM25_BOUND, st);   // inside the candidate span
-                if (deep) bm25_bound_deep_kernel<<<n_queries, kBdThreads, bd_smem, st>>>(p, c);
-                else bm25_bound_kernel<<<n_queries, kBdThreads, 0, st>>>(p, c);
+                if (deep) bm25_bound_deep_kernel<S><<<n_queries, kBdThreads, bd_smem, st>>>(p, c);
+                else bm25_bound_kernel<S><<<n_queries, kBdThreads, 0, st>>>(p, c);
                 EZR_LAUNCH_CHECK();
             }
             if (r0 > first && span < kPkMaxChunk) span *= 2;
@@ -744,8 +749,8 @@ static int pk_launch(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32
     }
     {
         ProfScope prof(EZR_PROF_BM25_RESCORE, st);
-        if (deep) bm25_rescore_deep_kernel<<<n_queries, kRsThreads, 0, st>>>(p, c, w.rows);
-        else bm25_rescore_kernel<<<n_queries, kRsThreads, 0, st>>>(p, c, out_scores, out_ids, out_counts);
+        if (deep) bm25_rescore_deep_kernel<S><<<n_queries, kRsThreads, 0, st>>>(p, c, (S*)w.rows);
+        else bm25_rescore_kernel<S><<<n_queries, kRsThreads, 0, st>>>(p, c, out_scores, out_ids, out_counts);
         EZR_LAUNCH_CHECK();
     }
     return EZR_OK;
@@ -858,6 +863,87 @@ static int rows_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32
     return EZR_OK;
 }
 
+// two-phase top-k, k <= 32: candidates from packed postings -> exact rescoring; overflowed queries (normally none)
+// go through the ordered kernel, restricted to ovf_list.  lists: the ordered kernel's [Q][ranges][k] partial lists
+// (scores, then ids at ids_off), followed by the two-phase workspace.
+template <typename S>
+static int pk_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t* q_terms, int n_queries, int k,
+                   const int32_t* q_group, int id_base, void* lists, size_t ids_off, int32_t* thr, S* out_scores,
+                   int32_t* out_ids, int32_t* out_counts, cudaStream_t st) {
+    int32_t* pi = reinterpret_cast<int32_t*>((char*)lists + ids_off);
+    const PkWorkspace w = pk_carve(thr, n_queries);
+    EZR_CUDA(cudaMemsetAsync(thr, 0, w.zero_bytes, st));
+    int rc = pk_launch<S>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, w, out_scores, out_ids, out_counts, st);
+    if (rc) return rc;
+    rc = bm25_launch<S>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, 0, lists, pi, w.thr_key, st, w.ovf_list,
+                        w.ovf_n);
+    if (rc) return rc;
+    const int n_cand = ix->n_ranges * k;
+    return merge_impl<S>((const S*)lists, pi, n_queries, n_cand, n_cand, k, id_base, out_scores, out_ids, out_counts,
+                         st, w.ovf_list, w.ovf_n);
+}
+
+// deep form, 32 < k <= kSelMaxK: candidates from packed postings -> exact scores in [Q][cap] rows -> the select
+// takes each top-k; overflowed queries (normally none) are then answered from their score rows
+template <typename S>
+static int pk_topk_deep(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t* q_terms, int n_queries, int k,
+                        const int32_t* q_group, int id_base, void* workspace, S* out_scores, int32_t* out_ids,
+                        int32_t* out_counts, cudaStream_t st) {
+    const int cap = pk_deep_list_cap(k);
+    const PkWorkspace w = pk_carve(workspace, n_queries, cap, true, sizeof(S));
+    const RowsWorkspace rw = rows_carve((char*)workspace + w.total, ix, n_queries, k);
+    EZR_CUDA(cudaMemsetAsync(workspace, 0, w.zero_bytes, st));
+    int rc = pk_launch<S>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, w, nullptr, nullptr, nullptr, st, true);
+    if (rc) return rc;
+    rc = launch_select<S>((const S*)w.rows, w.cand_ids, n_queries, cap, cap, 1, k, 1, nullptr, nullptr, id_base,
+                          out_scores, out_ids, out_counts, st);
+    if (rc) return rc;
+    // the host learns how many queries overflowed (one small copy + stream sync) to size the score-row pass
+    int32_t n_ovf = 0;
+    EZR_CUDA(cudaMemcpyAsync(&n_ovf, w.ovf_n, 4, cudaMemcpyDeviceToHost, st));
+    EZR_CUDA(cudaStreamSynchronize(st));
+    if (n_ovf == 0) return EZR_OK;
+    return rows_topk<S>(ix, q_ptr, q_terms, k, q_group, id_base, w.ovf_list, n_ovf, out_scores, out_ids, out_counts,
+                        rw, st);
+}
+
+// ezr_bm25_pack / ezr_bm25_pack_f32: W = the stored weight type, widened to double exactly
+template <typename W>
+static int bm25_pack_impl(const int32_t* post_doc, const W* post_w, int64_t n_postings, int32_t range_size,
+                          uint32_t* out_pk, int32_t* out_scale_log2, void* scratch16, cudaStream_t st) {
+    EZR_CHECK_ARG(kPkEnabled, "bm25_pack: this build's range size %d is not a power of two", kBmRange);
+    EZR_CHECK_ARG(range_size == kBmRange, "bm25_pack: range_size must be %d (got %d)", kBmRange, range_size);
+    EZR_CHECK_ARG(out_scale_log2 != nullptr && scratch16 != nullptr, "bm25_pack: NULL argument");
+    EZR_CHECK_ARG(n_postings >= 0 && n_postings < ((int64_t)1 << 31), "bm25_pack: n_postings out of range");
+    *out_scale_log2 = 0;
+    if (n_postings == 0) return EZR_OK;
+    unsigned long long* d = reinterpret_cast<unsigned long long*>(scratch16);
+    EZR_CUDA(cudaMemsetAsync(d, 0, 16, st));
+    bm25_wmax_kernel<W><<<sm_count() * 8, 256, 0, st>>>(post_w, n_postings, d);
+    EZR_LAUNCH_CHECK();
+    unsigned long long h[2];
+    EZR_CUDA(cudaMemcpyAsync(h, d, 16, cudaMemcpyDeviceToHost, st));
+    EZR_CUDA(cudaStreamSynchronize(st));
+    if (h[1] != 0ull) {
+        set_error("bm25_pack: negative or non-finite contribution; the two-phase path needs non-negative weights");
+        return EZR_ERR_INVALID;
+    }
+    double wmax;
+    memcpy(&wmax, &h[0], 8);
+    int e = 0;
+    if (wmax > 0.0) {
+        int ex;
+        frexp(wmax, &ex);                       // wmax < 2^ex
+        e = kPkWBits - 1 - ex;                  // wmax * 2^e < 2^(WBits-1): ceil() fits, sums of 2^(31-WBits) terms too
+    }
+    const double scale = ldexp(1.0, e);
+    bm25_pack_kernel<W><<<(unsigned)((n_postings + 255) / 256), 256, 0, st>>>(post_doc, post_w, n_postings, scale,
+                                                                             out_pk);
+    EZR_LAUNCH_CHECK();
+    *out_scale_log2 = e;
+    return EZR_OK;
+}
+
 }  // namespace ezr
 
 using namespace ezr;
@@ -906,37 +992,14 @@ int ezr_bm25_range_index(const int64_t* indptr, const int32_t* post_doc, int32_t
 
 int ezr_bm25_pack(const int32_t* post_doc, const double* post_w, int64_t n_postings, int32_t range_size,
                   uint32_t* out_pk, int32_t* out_scale_log2, void* scratch16, void* stream) {
-    EZR_CHECK_ARG(kPkEnabled, "bm25_pack: this build's range size %d is not a power of two", kBmRange);
-    EZR_CHECK_ARG(range_size == kBmRange, "bm25_pack: range_size must be %d (got %d)", kBmRange, range_size);
-    EZR_CHECK_ARG(out_scale_log2 != nullptr && scratch16 != nullptr, "bm25_pack: NULL argument");
-    EZR_CHECK_ARG(n_postings >= 0 && n_postings < ((int64_t)1 << 31), "bm25_pack: n_postings out of range");
-    cudaStream_t st = (cudaStream_t)stream;
-    *out_scale_log2 = 0;
-    if (n_postings == 0) return EZR_OK;
-    unsigned long long* d = reinterpret_cast<unsigned long long*>(scratch16);
-    EZR_CUDA(cudaMemsetAsync(d, 0, 16, st));
-    bm25_wmax_kernel<<<sm_count() * 8, 256, 0, st>>>(post_w, n_postings, d);
-    EZR_LAUNCH_CHECK();
-    unsigned long long h[2];
-    EZR_CUDA(cudaMemcpyAsync(h, d, 16, cudaMemcpyDeviceToHost, st));
-    EZR_CUDA(cudaStreamSynchronize(st));
-    if (h[1] != 0ull) {
-        set_error("bm25_pack: negative or non-finite contribution; the two-phase path needs non-negative weights");
-        return EZR_ERR_INVALID;
-    }
-    double wmax;
-    memcpy(&wmax, &h[0], 8);
-    int e = 0;
-    if (wmax > 0.0) {
-        int ex;
-        frexp(wmax, &ex);                       // wmax < 2^ex
-        e = kPkWBits - 1 - ex;                  // wmax * 2^e < 2^(WBits-1): ceil() fits, sums of 2^(31-WBits) terms too
-    }
-    const double scale = ldexp(1.0, e);
-    bm25_pack_kernel<<<(unsigned)((n_postings + 255) / 256), 256, 0, st>>>(post_doc, post_w, n_postings, scale, out_pk);
-    EZR_LAUNCH_CHECK();
-    *out_scale_log2 = e;
-    return EZR_OK;
+    return bm25_pack_impl<double>(post_doc, post_w, n_postings, range_size, out_pk, out_scale_log2, scratch16,
+                                  (cudaStream_t)stream);
+}
+
+int ezr_bm25_pack_f32(const int32_t* post_doc, const float* post_w, int64_t n_postings, int32_t range_size,
+                      uint32_t* out_pk, int32_t* out_scale_log2, void* scratch16, void* stream) {
+    return bm25_pack_impl<float>(post_doc, post_w, n_postings, range_size, out_pk, out_scale_log2, scratch16,
+                                 (cudaStream_t)stream);
 }
 
 int ezr_bm25_term_max(const int64_t* indptr, const uint32_t* post_pk, int32_t vocab, uint32_t* out_term_max,
@@ -980,7 +1043,7 @@ size_t ezr_bm25_topk_workspace(const ezr_bm25_index* ix, int32_t n_queries, int3
     // deep form: candidate lists and their score rows (Q * pk_deep_list_cap(k)), plus one block of score rows for
     // the queries that overflow them; otherwise blocks of score rows only
     const size_t rows = rows_carve(nullptr, ix, n_queries, k).total;
-    if (pk_deep_usable(ix, k)) return pk_carve(nullptr, n_queries, pk_deep_list_cap(k), true).total + rows;
+    if (pk_deep_usable(ix, k)) return pk_carve(nullptr, n_queries, pk_deep_list_cap(k), true, ss).total + rows;
     return rows;
 }
 
@@ -1013,19 +1076,11 @@ int ezr_bm25_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t*
         int32_t* pi = reinterpret_cast<int32_t*>((char*)workspace + align_up(n * ss, 256));
         int32_t* thr = reinterpret_cast<int32_t*>((char*)workspace + align_up(n * ss, 256) + align_up(n * 4, 256));
         if (pk_usable(ix, k)) {
-            // candidates from packed postings -> exact rescoring; overflowed queries (normally none) go through
-            // the ordered kernel below, restricted to ovf_list
-            const PkWorkspace w = pk_carve(thr, n_queries);
-            EZR_CUDA(cudaMemsetAsync(thr, 0, w.zero_bytes, st));
-            rc = pk_launch(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, w, (double*)out_scores, out_ids,
-                           out_counts, st);
-            if (rc) return rc;
-            rc = bm25_launch<double>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, 0, ps, pi, w.thr_key, st,
-                                     w.ovf_list, w.ovf_n);
-            if (rc) return rc;
-            const int n_cand = ix->n_ranges * k;
-            return merge_impl<double>((const double*)ps, pi, n_queries, n_cand, n_cand, k, id_base,
-                                      (double*)out_scores, out_ids, out_counts, st, w.ovf_list, w.ovf_n);
+            const size_t ids_off = align_up(n * ss, 256);
+            return f64 ? pk_topk<double>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, ps, ids_off, thr,
+                                         (double*)out_scores, out_ids, out_counts, st)
+                       : pk_topk<float>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, ps, ids_off, thr,
+                                        (float*)out_scores, out_ids, out_counts, st);
         }
         EZR_CUDA(cudaMemsetAsync(thr, 0, (size_t)n_queries * 4, st));
         rc = f64 ? bm25_launch<double>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, 0, ps, pi, thr, st)
@@ -1037,26 +1092,11 @@ int ezr_bm25_topk(const ezr_bm25_index* ix, const int32_t* q_ptr, const int32_t*
                    : merge_impl<float>((const float*)ps, pi, n_queries, n_cand, n_cand, k, id_base,
                                        (float*)out_scores, out_ids, out_counts, st);
     }
-    if (pk_deep_usable(ix, k)) {
-        // candidates from packed postings -> exact scores in [Q][cap] rows -> the select takes each top-k;
-        // overflowed queries (normally none) are then answered from their score rows
-        const int cap = pk_deep_list_cap(k);
-        const PkWorkspace w = pk_carve(workspace, n_queries, cap, true);
-        const RowsWorkspace rw = rows_carve((char*)workspace + w.total, ix, n_queries, k);
-        EZR_CUDA(cudaMemsetAsync(workspace, 0, w.zero_bytes, st));
-        rc = pk_launch(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, w, nullptr, nullptr, nullptr, st, true);
-        if (rc) return rc;
-        rc = launch_select<double>(w.rows, w.cand_ids, n_queries, cap, cap, 1, k, 1, nullptr, nullptr, id_base,
-                                   (double*)out_scores, out_ids, out_counts, st);
-        if (rc) return rc;
-        // the host learns how many queries overflowed (one small copy + stream sync) to size the score-row pass
-        int32_t n_ovf = 0;
-        EZR_CUDA(cudaMemcpyAsync(&n_ovf, w.ovf_n, 4, cudaMemcpyDeviceToHost, st));
-        EZR_CUDA(cudaStreamSynchronize(st));
-        if (n_ovf == 0) return EZR_OK;
-        return rows_topk<double>(ix, q_ptr, q_terms, k, q_group, id_base, w.ovf_list, n_ovf, (double*)out_scores,
-                                 out_ids, out_counts, rw, st);
-    }
+    if (pk_deep_usable(ix, k))
+        return f64 ? pk_topk_deep<double>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, workspace,
+                                          (double*)out_scores, out_ids, out_counts, st)
+                   : pk_topk_deep<float>(ix, q_ptr, q_terms, n_queries, k, q_group, id_base, workspace,
+                                         (float*)out_scores, out_ids, out_counts, st);
     const RowsWorkspace rw = rows_carve(workspace, ix, n_queries, k);
     return f64 ? rows_topk<double>(ix, q_ptr, q_terms, k, q_group, id_base, nullptr, n_queries, (double*)out_scores,
                                    out_ids, out_counts, rw, st)

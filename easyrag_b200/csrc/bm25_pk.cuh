@@ -1,4 +1,4 @@
-// Two-phase BM25 top-k (float64 Okapi indices with non-negative weights): included by bm25.cu.
+// Two-phase BM25 top-k (float64 Okapi and float32 bm25s indices with non-negative weights): included by bm25.cu.
 //
 // The ordered float64 accumulation of bm25_score_kernel pays one block barrier per query term to reproduce the
 // reference's sum order (retrievers.py:128-151 -> rank_bm25 get_scores adds term by term) for EVERY document,
@@ -8,7 +8,7 @@
 //                                  (doc-in-range | ceil(w * 2^e)), shared-memory integer atomics, NO ordering and
 //                                  no per-term barrier; documents that may reach the top-k are appended to a
 //                                  per-query candidate list.
-//   phase 2  bm25_rescore_kernel   every candidate's exact float64 score, terms added strictly in token order
+//   phase 2  bm25_rescore_kernel   every candidate's exact score (float64 or float32), terms added strictly in token order
 //                                  (binary search of the candidate in each term's posting segment), then the
 //                                  canonical top-k of the candidates.
 //
@@ -32,6 +32,22 @@
 // multiplied and the rescoring ate the gain.  So the kernel COMPLETES the relaxed crossers
 // inside the candidate kernel (binary search of each skipped token's postings for just those documents) and then
 // applies the exact test, so the candidate set and the bounds are those of a full pass (L = U = Q).
+//
+// Float32 scores (bm25s, Lucene idf log(1 + (N - df + 0.5)/(df + 0.5)) > 0, so every such index is monotone).  bm25s
+// adds a query's contributions with np.add.at token by token, so s(d) is a float32 sum rounded after every add
+// (u = 2^-24).  For m non-negative addends the sequential sum satisfies |s - R| <= gamma_{m-1} * R with
+// gamma_n = n*u / (1 - n*u).  The weights are widened to double (exactly) and packed with the same scale rule, so
+// S*w < 2^(kPkWBits-1) = 2^18 for every posting and S*R < m * 2^18.  Hence, with
+//   e(m) = ceil(gamma_{m-1} * m * 2^18) = ceil((m-1) * m * 2^18 / (2^24 - (m-1)))      (0 at m = 1, 14 at m = 30,
+//                                                                                      2^18 at kPkMaxTerms)
+//   Q(d) - m - e(m)  <=  S*s(d)  <=  Q(d) + e(m).
+// The float64 bracket above is the same statement with u = 2^-53: there gamma_{m-1} * m * 2^18 < 1 for every
+// m <= kPkMaxTerms, so e = 1.  Everything else carries over with e in place of that 1: B := G - m - e, a document
+// is kept when Q(d) >= B - e (S*s(d) >= B is then possible), the bound steps subtract m + e, and with skipped
+// tokens the relaxed crossing threshold is B - e - NE.  PkSlack<S>::e is that constant; the candidate and bound
+// kernels are instantiated per score type (the float64 instances compile to the code they had with the literal 1),
+// and phase 2 adds float32 contributions with __fadd_rn in token order from +0.0f (absent tokens add +0.0f, exact).
+// All integer quantities stay below 2^31: Q <= kPkMaxTerms * 2^18 = 2^30 and e(m) <= 2^18.
 #pragma once
 #include <type_traits>
 
@@ -84,6 +100,23 @@ constexpr int kPkGroup = kPkThreads / 32;                 // lanes per group: 32
 static_assert(kPkThreads % 32 == 0 && kPkThreads >= 64 && (kPkGroup & (kPkGroup - 1)) == 0, "bad EZR_BM25_PK_THREADS");
 static_assert(kBmRange % (4 * kPkThreads) == 0, "range must be a multiple of 4 * EZR_BM25_PK_THREADS");
 
+// e(m) of the bracket  Q - m - e <= S*s <= Q + e  for a query of m tokens (header): the rounding error of the
+// sequential sum in the score type, in units of 1/S.
+template <typename S> struct PkSlack;
+template <> struct PkSlack<double> {
+    static __host__ __device__ constexpr int e(int) { return 1; }
+};
+template <> struct PkSlack<float> {
+    static __host__ __device__ constexpr int e(int m) {
+        const int64_t n = m > 1 ? m - 1 : 0;              // gamma_{m-1} = n*2^-24 / (1 - n*2^-24), exactly in integers
+        const int64_t num = n * m * ((int64_t)1 << (kPkWBits - 1)), den = ((int64_t)1 << 24) - n;
+        return (int)((num + den - 1) / den);
+    }
+};
+static_assert(kPkWBits != 19 || (PkSlack<float>::e(1) == 0 && PkSlack<float>::e(2) == 1 &&
+                                 PkSlack<float>::e(30) == 14 && PkSlack<float>::e(kPkMaxTerms) == 262144),
+              "float32 slack e(m)");
+
 struct PkParams {
     const uint32_t* post_pk;   // [n_postings]
     int32_t* thr_q;            // [Q] running bound B (integer domain), zeroed per call
@@ -101,11 +134,13 @@ struct PkParams {
 };
 
 // ---- index build: largest weight (as bits; non-negative doubles order like their bit patterns) + validity ----
-__global__ void bm25_wmax_kernel(const double* __restrict__ w, int64_t n, unsigned long long* __restrict__ out) {
+// W: the stored weight type; float32 weights are widened to double, which is exact.
+template <typename W>
+__global__ void bm25_wmax_kernel(const W* __restrict__ w, int64_t n, unsigned long long* __restrict__ out) {
     unsigned long long mx = 0ull;
     int bad = 0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const double v = w[i];
+        const double v = (double)w[i];
         if (!(v >= 0.0) || isinf(v)) bad = 1;
         else mx = max(mx, (unsigned long long)__double_as_longlong(v));
     }
@@ -120,11 +155,12 @@ __global__ void bm25_wmax_kernel(const double* __restrict__ w, int64_t n, unsign
     }
 }
 
-__global__ void bm25_pack_kernel(const int32_t* __restrict__ post_doc, const double* __restrict__ w, int64_t n,
+template <typename W>
+__global__ void bm25_pack_kernel(const int32_t* __restrict__ post_doc, const W* __restrict__ w, int64_t n,
                                  double scale, uint32_t* __restrict__ out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const double x = ceil(__dmul_rn(w[i], scale));       // exact product (power of two), exact ceil
+    const double x = ceil(__dmul_rn((double)w[i], scale));   // exact product (power of two), exact ceil
     out[i] = ((uint32_t)(post_doc[i] & (kBmRange - 1)) << kPkWBits) | (uint32_t)x;
 }
 
@@ -240,7 +276,8 @@ constexpr int kPkPiece = 32 * kPkUnroll;                 // postings per work it
 // accumulators), the candidate list lives in dynamic shared memory behind the accumulators, the capacities are
 // pk_deep_local_cap / pk_deep_list_cap, and the in-range raise is a select over the range's candidates.  (A kernel
 // template, not a body inlined into two kernels: inlining changes the k <= 32 instance's register allocation.)
-template <bool DEEP>
+// S: the index's score type, which fixes the slack e(m) of the bracket (PkSlack).
+template <bool DEEP, typename S>
 __global__ void __launch_bounds__(kPkThreads, DEEP ? 4 : EZR_BM25_PK_MINB)
 bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
     extern __shared__ __align__(16) unsigned char pk_smem_raw[];
@@ -261,6 +298,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
         if (tid == 0) c.ovf[q] = 1;
         return;
     }
+    const int es = PkSlack<S>::e(m);                     // e(m): keep Q >= B - e, bounds step down by m + e
     const int rbase = r * kBmRange;
     const uint32_t* __restrict__ pk = c.post_pk;
     const int want = p.q_group ? p.q_group[q] : -1;
@@ -311,7 +349,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
     const int ne = s_ne;
     // crossing test in one unsigned compare: old < tq <= old + wq  <=>  tq - 1 - old < wq  (wraps to a huge value
     // when old >= tq; without a bound tq1 = 2^32-1: ~old is never below a packed weight)
-    const uint32_t tq1 = track ? (uint32_t)max(bound - 1 - ne, 1) - 1u : 0xffffffffu;
+    const uint32_t tq1 = track ? (uint32_t)max(bound - es - ne, 1) - 1u : 0xffffffffu;
     // Lanes without a posting add 0 to a private spare slot behind the accumulators (no branch around the atomic,
     // no same-address serialisation); crossings are rare: the caller votes and only then takes the push path.
     const uint32_t spare = (uint32_t)(kBmRange + lane);
@@ -394,7 +432,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
     }
     __syncthreads();                                     // every contribution of this (query, range) is in acc
 
-    const int slack = m + 1;
+    const int slack = m + es;
     if (!track) {
         // No bound yet (first ranges of a query): k-th largest of 32 disjoint group maxima = G, then compact.
         constexpr int kPer = kBmRange / kPkThreads;
@@ -447,7 +485,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
         }
         const int g = s_thr;
         const int bl = g > 0 ? g - slack : 0;            // B from this range alone
-        const uint32_t tl = (uint32_t)max(bl - 1, 1);
+        const uint32_t tl = (uint32_t)max(bl - es, 1);
         __syncthreads();                                 // s_wi is reused as the candidate list
         if (tmax >= tl) {
 #pragma unroll 4
@@ -468,9 +506,9 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
         if (tid == 0) c.ovf[q] = 1;
         return;
     }
-    // Skipped (non-essential) tokens: the documents above crossed the RELAXED threshold B - 1 - NE on their essential
+    // Skipped (non-essential) tokens: the documents above crossed the RELAXED threshold B - e - NE on their essential
     // tokens alone.  Complete their sums here -- one thread per (document, skipped token) binary-searches the token's
-    // packed postings of this range -- so that the test below is the exact one (Q >= B - 1) and the candidates carry
+    // packed postings of this range -- so that the test below is the exact one (Q >= B - e) and the candidates carry
     // their full integer score: the candidate set and the bound updates are then exactly those of a pass that read
     // every posting, and only the handful of near-candidates pays for the long lists.
     const uint32_t nm = (uint32_t)s_nm;
@@ -499,7 +537,7 @@ bm25_cand_kernel(const Bm25Params p, const PkParams c, const int r_begin) {
     for (int i = tid; i < n; i += kPkThreads) {
         const int dl = s_wi[i];
         const uint32_t mine = acc[dl];
-        if (nm != 0u && (int)mine < bound - 1) continue;  // crossed only the relaxed threshold
+        if (nm != 0u && (int)mine < bound - es) continue;  // crossed only the relaxed threshold
         const int slot = atomicAdd(c.cand_cnt + q, 1);
         if (slot < list_cap) {
             c.cand_ids[(int64_t)q * list_cap + slot] = rbase + dl;
@@ -537,7 +575,7 @@ constexpr int kBdThreads = 128;
 
 // DEEP: the list has pk_deep_list_cap(k) slots, staged in dynamic shared memory, and the k-th largest lower bound
 // comes from a radix select instead of pairwise ranks.
-template <bool DEEP>
+template <bool DEEP, typename S>
 __device__ __forceinline__ void bm25_bound_body(const Bm25Params& p, const PkParams& c) {
     __shared__ int s_q_fixed[DEEP ? 1 : kPkListCap];
     __shared__ int s_u_fixed[DEEP ? 1 : kPkListCap];
@@ -582,9 +620,10 @@ __device__ __forceinline__ void bm25_bound_body(const Bm25Params& p, const PkPar
     __syncthreads();
     const int qs = p.q_ptr[q];
     const int m = p.q_ptr[q + 1] - qs;
-    const int b = max(s_kth - (m + 1), c.thr_q[q]);      // the k-th largest LOWER bound is a valid bound
+    const int es = PkSlack<S>::e(m);
+    const int b = max(s_kth - (m + es), c.thr_q[q]);     // the k-th largest LOWER bound is a valid bound
     for (int i = tid; i < n; i += kBdThreads) {
-        if (s_u[i] >= b - 1) {                           // keep what may still reach it: UPPER bounds decide
+        if (s_u[i] >= b - es) {                          // keep what may still reach it: UPPER bounds decide
             const int pos = atomicAdd(&s_n2, 1);
             c.cand_q[(int64_t)q * list_cap + pos] = s_q[i];
             c.cand_u[(int64_t)q * list_cap + pos] = s_u[i];
@@ -597,8 +636,8 @@ __device__ __forceinline__ void bm25_bound_body(const Bm25Params& p, const PkPar
         c.cand_cnt[q] = s_n2;
     }
     // Non-essential tokens for the ranges still to come (first 32 tokens; one warp): ascending by term maximum,
-    // the longest prefix whose sum stays within kPkNeNum/kPkNeDen of b - 1.
-    if (kPkNeNum > 0 && c.term_max != nullptr && tid < 32 && b > 1) {
+    // the longest prefix whose sum stays within kPkNeNum/kPkNeDen of b - e.
+    if (kPkNeNum > 0 && c.term_max != nullptr && tid < 32 && b > es) {
         const int lane = tid;
         uint32_t gm = 0xffffffffu;                       // lanes without a token sort last and are never chosen
         bool have = false;
@@ -619,7 +658,7 @@ __device__ __forceinline__ void bm25_bound_body(const Bm25Params& p, const PkPar
             const bool hj = __shfl_sync(0xffffffffu, have ? 1 : 0, j) != 0;
             if (hj && r <= rank) pre += o;
         }
-        const unsigned long long budget = (unsigned long long)(b - 1) * kPkNeNum / kPkNeDen;
+        const unsigned long long budget = (unsigned long long)(b - es) * kPkNeNum / kPkNeDen;
         const bool skip = have && pre <= budget;
         const uint32_t mask = __ballot_sync(0xffffffffu, skip);
         unsigned long long ne = skip ? (unsigned long long)gm : 0ull;
@@ -632,14 +671,16 @@ __device__ __forceinline__ void bm25_bound_body(const Bm25Params& p, const PkPar
     }
 }
 
+template <typename S>
 __global__ void __launch_bounds__(kBdThreads)
 bm25_bound_kernel(const Bm25Params p, const PkParams c) {
-    bm25_bound_body<false>(p, c);
+    bm25_bound_body<false, S>(p, c);
 }
 
+template <typename S>
 __global__ void __launch_bounds__(kBdThreads)
 bm25_bound_deep_kernel(const Bm25Params p, const PkParams c) {
-    bm25_bound_body<true>(p, c);
+    bm25_bound_body<true, S>(p, c);
 }
 
 inline size_t pk_deep_bound_smem(int k) { return (size_t)(kPkHist + 3 * pk_deep_list_cap(k)) * 4; }
@@ -651,11 +692,16 @@ constexpr int kRsU = 4;        // candidates a warp scores at once (independent 
 
 // DEEP: out_scores is a [Q][pk_deep_list_cap(k)] row of exact scores beside the candidate ids (ids past the
 // query's candidates set to -1), from which the caller's select takes the canonical top-k.
-template <bool DEEP>
+// S: the index's score type; contributions of that type are added with its round-to-nearest add.
+template <typename S> __device__ __forceinline__ S add_rn(S a, S b);
+template <> __device__ __forceinline__ double add_rn<double>(double a, double b) { return __dadd_rn(a, b); }
+template <> __device__ __forceinline__ float add_rn<float>(float a, float b) { return __fadd_rn(a, b); }
+
+template <bool DEEP, typename S>
 __device__ __forceinline__ void bm25_rescore_body(const Bm25Params& p, const PkParams& c,
-                                                  double* __restrict__ out_scores, int32_t* __restrict__ out_ids,
+                                                  S* __restrict__ out_scores, int32_t* __restrict__ out_ids,
                                                   int32_t* __restrict__ out_counts) {
-    __shared__ double s_sc[DEEP ? 1 : kPkListCap];
+    __shared__ S s_sc[DEEP ? 1 : kPkListCap];
     __shared__ int s_id[DEEP ? 1 : kPkListCap];
     __shared__ int s_t[kRsTok];
     __shared__ int s_base[kRsTok];
@@ -677,23 +723,23 @@ __device__ __forceinline__ void bm25_rescore_body(const Bm25Params& p, const PkP
         s_base[j] = ok ? (int)p.indptr[t] : 0;
     }
     __syncthreads();
-    const double* __restrict__ post_w = reinterpret_cast<const double*>(p.post_w);
+    const S* __restrict__ post_w = reinterpret_cast<const S*>(p.post_w);
     // A warp scores kRsU candidates at once (lane = token): the kRsU binary searches of a lane are independent, so
     // their loads are in flight together -- the kernel is bound by the latency of those dependent L2 reads, not by
     // their count.  The sums stay per candidate, in token order.
     for (int cb = warp * kRsU; cb < n; cb += (kRsThreads / 32) * kRsU) {
         int doc[kRsU];
-        double s[kRsU];
+        S s[kRsU];
 #pragma unroll
         for (int u = 0; u < kRsU; ++u) {
             doc[u] = cb + u < n ? c.cand_ids[(int64_t)q * list_cap + cb + u] : -1;
-            s[u] = 0.0;
+            s[u] = (S)0;
         }
         for (int c0 = 0; c0 < m; c0 += 32) {
             const int j = c0 + lane;
-            double wv[kRsU];
+            S wv[kRsU];
 #pragma unroll
-            for (int u = 0; u < kRsU; ++u) wv[u] = 0.0;
+            for (int u = 0; u < kRsU; ++u) wv[u] = (S)0;
             int t = -1, base = 0;
             if (j < m) {
                 if (j < kRsTok) { t = s_t[j]; base = s_base[j]; }
@@ -738,7 +784,7 @@ __device__ __forceinline__ void bm25_rescore_body(const Bm25Params& p, const PkP
             const int cnt = min(32, m - c0);
             for (int jj = 0; jj < cnt; ++jj) {
 #pragma unroll
-                for (int u = 0; u < kRsU; ++u) s[u] = __dadd_rn(s[u], __shfl_sync(0xffffffffu, wv[u], jj));   // token order
+                for (int u = 0; u < kRsU; ++u) s[u] = add_rn<S>(s[u], __shfl_sync(0xffffffffu, wv[u], jj));   // token order
             }
         }
         if (lane == 0) {
@@ -757,12 +803,12 @@ __device__ __forceinline__ void bm25_rescore_body(const Bm25Params& p, const PkP
     }
     __syncthreads();
     for (int i = tid; i < n; i += kRsThreads) {
-        const double ms = s_sc[i];
+        const S ms = s_sc[i];
         const int mi = s_id[i];
-        if (ms > 0.0) {                                  // retrievers.py:195-196: only positive scores qualify
+        if (ms > (S)0) {                                 // retrievers.py:195-196: only positive scores qualify
             atomicAdd(&s_pos, 1);
             int rank = 0;
-            for (int j = 0; j < n; ++j) rank += better<double>(s_sc[j], s_id[j], ms, mi) ? 1 : 0;
+            for (int j = 0; j < n; ++j) rank += better<S>(s_sc[j], s_id[j], ms, mi) ? 1 : 0;
             if (rank < p.k) {
                 out_scores[(int64_t)q * p.k + rank] = ms;
                 out_ids[(int64_t)q * p.k + rank] = mi + p.id_base;
@@ -772,21 +818,23 @@ __device__ __forceinline__ void bm25_rescore_body(const Bm25Params& p, const PkP
     __syncthreads();
     const int have = min(s_pos, p.k);
     for (int i = have + tid; i < p.k; i += kRsThreads) {
-        out_scores[(int64_t)q * p.k + i] = ScoreTraits<double>::lowest();
+        out_scores[(int64_t)q * p.k + i] = ScoreTraits<S>::lowest();
         out_ids[(int64_t)q * p.k + i] = -1;
     }
     if (tid == 0) out_counts[q] = have;
 }
 
+template <typename S>
 __global__ void __launch_bounds__(kRsThreads)
-bm25_rescore_kernel(const Bm25Params p, const PkParams c, double* __restrict__ out_scores,
+bm25_rescore_kernel(const Bm25Params p, const PkParams c, S* __restrict__ out_scores,
                     int32_t* __restrict__ out_ids, int32_t* __restrict__ out_counts) {
-    bm25_rescore_body<false>(p, c, out_scores, out_ids, out_counts);
+    bm25_rescore_body<false, S>(p, c, out_scores, out_ids, out_counts);
 }
 
+template <typename S>
 __global__ void __launch_bounds__(kRsThreads)
-bm25_rescore_deep_kernel(const Bm25Params p, const PkParams c, double* __restrict__ rows) {
-    bm25_rescore_body<true>(p, c, rows, nullptr, nullptr);
+bm25_rescore_deep_kernel(const Bm25Params p, const PkParams c, S* __restrict__ rows) {
+    bm25_rescore_body<true, S>(p, c, rows, nullptr, nullptr);
 }
 
 }  // namespace ezr

@@ -168,6 +168,11 @@ class Bm25Index:
 
     Global statistics (idf, avgdl) always come from the whole corpus so that a row-sharded index
     scores exactly like the unsharded one (SURVEY.md 8(e)).
+
+    ``packed``: build the 4-byte packed postings that let ``ezr_bm25_topk`` run the two-phase path (integer
+    candidate pass + exact rescoring) for 1 <= k <= 1024.  ``None`` (default) packs float64 (Okapi) indexes and
+    leaves float32 (bm25s) ones on the ordered kernel; ``True`` packs either type; ``False`` packs neither.  Results
+    are the same bytes either way.
     """
 
     def __init__(self, stats: Bm25Stats, device=None, doc_lo: int = 0, doc_hi: Optional[int] = None,
@@ -236,23 +241,23 @@ class Bm25Index:
     def _build_packed(self):
         """4-byte packed postings for the candidate pass of ``ezr_bm25_topk`` (derived data, never stored on disk).
 
-        Only float64 indices with non-negative contributions qualify; ``EASYRAG_B200_BM25_PACKED=0`` keeps the
-        ordered single-pass kernel (A/B measurements)."""
+        Only indices with non-negative contributions qualify.  With ``packed=None`` float64 indices are packed
+        unless ``EASYRAG_B200_BM25_PACKED=0`` (keeps the ordered single-pass kernel, A/B measurements) and float32
+        (bm25s) ones are not; ``packed=True`` packs both (float32 weights through ``ezr_bm25_pack_f32``)."""
         self.post_pk, self.pk_scale_log2, self.term_max = None, 0, None
         want = getattr(self, "_packed_opt", None)
         if want is None:
-            want = os.environ.get("EASYRAG_B200_BM25_PACKED", "1") != "0"
-        if (not want or self.score_type != _lib.F64 or not self.monotone or self.n_postings == 0
-                or _lib.lib().ezr_bm25_cand_capacity() == 0):
+            want = self.score_type == _lib.F64 and os.environ.get("EASYRAG_B200_BM25_PACKED", "1") != "0"
+        if not want or not self.monotone or self.n_postings == 0 or _lib.lib().ezr_bm25_cand_capacity() == 0:
             return
         import ctypes
+        pack = _lib.lib().ezr_bm25_pack if self.score_type == _lib.F64 else _lib.lib().ezr_bm25_pack_f32
         with torch.cuda.device(self.device):
             pk = torch.empty(self.n_postings, dtype=torch.int32, device=self.device)
             scratch = torch.empty(2, dtype=torch.int64, device=self.device)
             e = ctypes.c_int32(0)
-            _lib.check(_lib.lib().ezr_bm25_pack(_lib.ptr(self.post_doc), _lib.ptr(self.post_w), self.n_postings,
-                                                _lib.BM25_RANGE, _lib.ptr(pk), ctypes.byref(e), _lib.ptr(scratch),
-                                                _lib.stream_ptr()), "ezr_bm25_pack")
+            _lib.check(pack(_lib.ptr(self.post_doc), _lib.ptr(self.post_w), self.n_postings, _lib.BM25_RANGE,
+                            _lib.ptr(pk), ctypes.byref(e), _lib.ptr(scratch), _lib.stream_ptr()), "ezr_bm25_pack")
             # per-term maximum of the packed weights: lets the candidate pass skip a query's lowest-weight terms
             tmax = torch.empty(self.vocab, dtype=torch.int32, device=self.device)
             _lib.check(_lib.lib().ezr_bm25_term_max(_lib.ptr(self.indptr), _lib.ptr(pk), self.vocab, _lib.ptr(tmax),
@@ -275,8 +280,8 @@ class Bm25Index:
         self._struct = s
 
     def ordered_view(self) -> "Bm25Index":
-        """The same device arrays without the packed postings: ``ezr_bm25_topk`` then runs the ordered float64
-        kernel.  Two independent kernel paths over one index = a full-size self-check (bench.py --self-check)."""
+        """The same device arrays without the packed postings: ``ezr_bm25_topk`` then runs the ordered kernel (float64
+        or float32).  Two independent kernel paths over one index = a full-size self-check (bench.py --self-check)."""
         import copy
         v = copy.copy(self)
         v._packed_opt = False

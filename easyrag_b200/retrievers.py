@@ -291,12 +291,15 @@ def _encode_corpus(token_lists: Sequence[Sequence[str]]):
 
 
 class BM25Retriever(BaseRetriever):
-    """retrievers.py:80-220: jieba-tokenised BM25 (Okapi fp64 / bm25s fp32), k1=1.5 b=0.75 eps=0.25."""
+    """retrievers.py:80-220: jieba-tokenised BM25 (Okapi fp64 / bm25s fp32), k1=1.5 b=0.75 eps=0.25.
+
+    ``packed``: as :class:`Bm25Index` -- ``None`` packs the postings of an Okapi index only, ``True`` also those of a
+    bm25s index (its top-k then runs the two-phase path); the results are the same either way."""
 
     def __init__(self, nodes: List[BaseNode], tokenizer: Optional[Callable[[str], List[str]]],
                  similarity_top_k: int = DEFAULT_SIMILARITY_TOP_K, callback_manager=None, objects=None,
                  object_map: Optional[dict] = None, verbose: bool = False, stopwords: List[str] = [""],
-                 embed_type: int = 0, bm25_type: int = 0, device="cuda") -> None:
+                 embed_type: int = 0, bm25_type: int = 0, device="cuda", packed: Optional[bool] = None) -> None:
         self._nodes = nodes
         self._tokenizer = tokenizer
         self._similarity_top_k = similarity_top_k
@@ -307,7 +310,7 @@ class BM25Retriever(BaseRetriever):
         self.k1, self.b, self.epsilon = K1, B, EPSILON
         self._device = device
         self._vocab, tokens, doc_ptr = _encode_corpus(self._corpus)
-        self.bm25 = self._build(tokens, doc_ptr, len(self._vocab))
+        self.bm25 = self._build(tokens, doc_ptr, len(self._vocab), packed=packed)
         self.filter_dict = None
         self.stopwords = stopwords
         self._groups = _GroupTable(self._nodes)
@@ -342,7 +345,8 @@ class BM25Retriever(BaseRetriever):
     def from_defaults(cls, index=None, nodes: Optional[List[BaseNode]] = None, docstore=None,
                       tokenizer: Optional[Callable[[str], List[str]]] = None,
                       similarity_top_k: int = DEFAULT_SIMILARITY_TOP_K, verbose: bool = False,
-                      stopwords: List[str] = [""], embed_type: int = 0, bm25_type: int = 0) -> "BM25Retriever":
+                      stopwords: List[str] = [""], embed_type: int = 0, bm25_type: int = 0,
+                      packed: Optional[bool] = None) -> "BM25Retriever":
         if sum(bool(val) for val in [index, nodes, docstore]) != 1:
             raise ValueError("Please pass exactly one of index, nodes, or docstore.")
         if index is not None:
@@ -351,7 +355,7 @@ class BM25Retriever(BaseRetriever):
             nodes = cast(List[BaseNode], list(docstore.docs.values()))
         assert nodes is not None, "Please pass exactly one of index, nodes, or docstore."
         return cls(nodes=nodes, tokenizer=tokenizer, similarity_top_k=similarity_top_k, verbose=verbose,
-                   stopwords=stopwords, embed_type=embed_type, bm25_type=bm25_type)
+                   stopwords=stopwords, embed_type=embed_type, bm25_type=bm25_type, packed=packed)
 
     def _apply_filter(self):
         doc_group, want = self._groups.resolve(self.filter_dict if self.filter_dict else None)

@@ -77,9 +77,10 @@ typedef struct ezr_bm25_index {
     const uint32_t* range_off; /* [vocab*(n_ranges+1)] */
     const int32_t* doc_group;  /* [n_docs] metadata class of each document, or NULL */
     int32_t monotone;          /* 1 if every post_w >= 0 (no negative idf): enables crossing-based selection */
-    int32_t pk_scale_log2;     /* e of ezr_bm25_pack (informational) */
-    const uint32_t* post_pk;   /* [n_postings] packed postings from ezr_bm25_pack, or NULL: enables the two-phase
-                                  top-k (integer candidate pass + exact float64 rescoring) for F64 / monotone / k<=32 */
+    int32_t pk_scale_log2;     /* e of ezr_bm25_pack / ezr_bm25_pack_f32 (informational) */
+    const uint32_t* post_pk;   /* [n_postings] packed postings from ezr_bm25_pack (F64 post_w) or ezr_bm25_pack_f32
+                                  (F32 post_w), or NULL: enables the two-phase top-k (integer candidate pass + exact
+                                  rescoring in the index's score type) for a monotone index */
     const uint32_t* term_max;  /* [vocab] from ezr_bm25_term_max, or NULL: lets the candidate pass skip the posting
                                   lists of a query's lowest-weight terms (MaxScore); results are unchanged */
 } ezr_bm25_index;
@@ -134,6 +135,11 @@ int ezr_bm25_shard_copy(const int64_t* first, const int64_t* indptr_local, const
 int ezr_bm25_pack(const int32_t* post_doc, const double* post_w, int64_t n_postings, int32_t range_size,
                   uint32_t* out_pk, int32_t* out_scale_log2, void* scratch16, void* stream);
 
+/* The same packed postings from float32 (bm25s) weights, widened to double exactly; the same scale rule and checks.
+ * With them ezr_bm25_topk rescores candidates as float32 sums in token order, bit-identical to bm25s get_scores. */
+int ezr_bm25_pack_f32(const int32_t* post_doc, const float* post_w, int64_t n_postings, int32_t range_size,
+                      uint32_t* out_pk, int32_t* out_scale_log2, void* scratch16, void* stream);
+
 /* out_term_max[t] = largest packed weight among term t's postings (0 for an empty list). */
 int ezr_bm25_term_max(const int64_t* indptr, const uint32_t* post_pk, int32_t vocab, uint32_t* out_term_max,
                       void* stream);
@@ -160,8 +166,9 @@ int ezr_bm25_cand_capacity(void);
  * Only documents with score > 0 qualify (retrievers.py:195-196); q_group[i] >= 0 additionally requires
  * doc_group[d] == q_group[i] (filter_dict, retrievers.py:198-202); -1 = no filter.
  * Outputs: out_scores[Q*k] (double/float per index->score_type), out_ids[Q*k] (-1 padded), out_counts[Q].
- * k <= 32 runs fused (accumulators never leave shared memory).  32 < k <= 1024 on a float64 index with non-negative
- * weights and packed postings runs the deep form of the two-phase path: its candidate lists hold 4k + 1024 entries
+ * k <= 32 runs fused (accumulators never leave shared memory); with packed postings on a monotone index (float64,
+ * or float32 packed by ezr_bm25_pack_f32) it runs the two-phase path.  32 < k <= 1024 on such an index
+ * runs the deep form of the two-phase path: its candidate lists hold 4k + 1024 entries
  * per query, and a query that overflows them (or one list of 2k + 512 for a range of 8192 documents) is answered
  * from its score row.  That path reads the number of such queries back to the host once per call (a 4-byte copy
  * and a stream synchronisation), so it cannot be captured into a CUDA graph.  Every other k > 32 case takes the
