@@ -66,6 +66,9 @@ SIGNATURES = {
     "ezr_bm25_topk_workspace": (_sz, [_IX, _i32, _i32]),
     "ezr_bm25_topk": (C.c_int, [_IX, _p, _p, _i32, _i32, _p, _i32, _p, _p, _p, _p, _sz, _p]),
     "ezr_bm25_scores": (C.c_int, [_IX, _p, _p, _i32, _p, _p]),
+    "ezr_bm25_extract_caps": (C.c_int, [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "ezr_bm25_extract": (C.c_int, [_p, _p, _p, _i32, _p, _p, _p, _p, _i32, _i32, _i32, _p, _i64, _p, _dbl, _dbl,
+                                   _dbl, _dbl, _i32, _p, _p, _p, _p]),
     "ezr_select_rows_workspace": (_sz, [_i32, _i64, _i32, _i32]),
     "ezr_select_rows": (C.c_int, [_p, _i32, _i32, _i64, _i64, _i32, _i32, _p, _p, _i32, _p, _p, _p, _p, _sz, _p]),
     "ezr_merge_topk_workspace": (_sz, [_i32, _i32, _i32, _i32]),

@@ -7,6 +7,7 @@ arithmetic is in easyrag_b200/csrc/*.cu.
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from typing import Optional, Sequence, Tuple
 
@@ -192,6 +193,136 @@ def bm25_scores(index: Bm25Index, q_ptr: torch.Tensor, q_terms: torch.Tensor, st
     with torch.cuda.device(dev):
         _lib.check(L.ezr_bm25_scores(index.struct, _lib.ptr(qp), _lib.ptr(qt), nq, _lib.ptr(out),
                                      _lib.stream_ptr(stream)), "ezr_bm25_scores")
+    return out
+
+
+@dataclass
+class Extract:
+    keep: torch.Tensor               # uint8 [S]: sentence kept
+    counts: torch.Tensor             # int32 [G]: sentences kept; -1 = the group has no sentences
+    scores: Optional[torch.Tensor]   # [S] float64 (Okapi) / float32 (bm25s), when asked for
+
+
+def extract_caps() -> Tuple[int, int]:
+    """(tokens, sentences) of the largest group :func:`bm25_extract` answers in its one launch."""
+    import ctypes
+    t, s = ctypes.c_int32(0), ctypes.c_int32(0)
+    _lib.check(_lib.lib().ezr_bm25_extract_caps(ctypes.byref(t), ctypes.byref(s)), "ezr_bm25_extract_caps")
+    return t.value, s.value
+
+
+_LOG_HALF: dict = {}      # device -> float64 L[j] = math.log(j + 0.5)
+_IDF_BM25S: dict = {}     # device -> float32 bm25s idf of (N, df) at N*(N+1)/2 + df, 0 <= df <= N
+
+
+def log_half_table(n: int):
+    """float64 L[j] = math.log(j + 0.5), j < n: rank_bm25's idf of df n among N documents is L[N - n] - L[n] bit for
+    bit, because N - n + 0.5 is exact."""
+    import numpy as np
+    return np.array([math.log(j + 0.5) for j in range(n)], dtype=np.float64)
+
+
+def _log_half(n: int, dev) -> torch.Tensor:
+    t = _LOG_HALF.get(dev)
+    if t is None or t.numel() < n:
+        t = torch.from_numpy(log_half_table(max(n, 2 * (t.numel() if t is not None else 0), 1024))).to(dev)
+        _LOG_HALF[dev] = t
+    return t
+
+
+def _bm25s_idf_table(max_n: int, dev) -> torch.Tensor:
+    from .index import bm25s_idf
+    t = _IDF_BM25S.get(dev)
+    have = 0 if t is None else int((math.isqrt(8 * t.numel() + 1) - 1) // 2)    # t covers N < have
+    if have <= max_n:
+        top = max(max_n + 1, 2 * have, 256)
+        vals = [0.0 if d == 0 else bm25s_idf(n, d) for n in range(top) for d in range(n + 1)]
+        t = torch.tensor(vals, dtype=torch.float64).to(torch.float32).to(dev)
+        _IDF_BM25S[dev] = t
+    return t
+
+
+def _select_host(scores, chars, ctx_chars: int, rate: float):
+    """The reference's walk (compressors.py:44-50) in the canonical order: score descending, then index descending."""
+    import numpy as np
+    order = np.argsort(scores, kind="stable")[::-1]
+    run = np.cumsum(np.asarray(chars, dtype=np.int64)[order])
+    hit = np.nonzero(run >= ctx_chars * rate)[0]
+    keep = np.zeros(len(scores), dtype=np.uint8)
+    keep[order[:(hit[0] + 1) if hit.size else len(order)]] = 1
+    return keep
+
+
+def bm25_extract(sent_ptr, tok_ptr, tokens, sent_chars, ctx_chars, q_ptr, q_tokens, vocab: int, rate: float = 0.5,
+                 bm25_type: int = 0, k1: Optional[float] = None, b: Optional[float] = None,
+                 epsilon: Optional[float] = None, scores: bool = False, device="cuda", stream=None) -> Extract:
+    """BM25-Extract over a batch of groups (``ezr_bm25_extract``): group g is a context's sentences
+    ``[sent_ptr[g], sent_ptr[g+1])`` with tokens ``tokens[tok_ptr[s]:tok_ptr[s+1]]`` (ids < ``vocab``, one vocabulary for
+    the batch) and its query ``q_tokens[q_ptr[g]:q_ptr[g+1]]`` (-1 = unknown).  Each group's scores are those of
+    ``BM25Retriever.get_scores(query, sentences)``; ``keep`` marks the sentences the reference compressor keeps.
+
+    ``sent_ptr`` / ``tok_ptr`` are read on the host (pass CPU tensors or arrays: the call then does not synchronise).
+    Groups within :func:`extract_caps` run in one launch; larger ones are answered one by one through a throw-away
+    index and ``ezr_bm25_scores`` with the selection on the host, which synchronises."""
+    import numpy as np
+    from .index import B as B_, EPSILON as EPS_, K1 as K1_, Bm25Stats
+    k1 = K1_ if k1 is None else k1
+    b = B_ if b is None else b
+    epsilon = EPS_ if epsilon is None else epsilon
+    if bm25_type not in (0, 1):
+        raise ValueError("bm25_type must be 0 (BM25Okapi) or 1 (bm25s)")
+    dev = torch.device(device)
+    sp = torch.as_tensor(sent_ptr).to(torch.int64).cpu()
+    tp = torch.as_tensor(tok_ptr).to(torch.int64).cpu()
+    G = sp.numel() - 1
+    n_sent = sp[1:] - sp[:-1]
+    n_tok = tp[sp[1:]] - tp[sp[:-1]]
+    cap_t, cap_s = extract_caps()
+    over = (n_tok > cap_t) | (n_sent > cap_s)
+    inside = ~over
+    max_t = int(n_tok[inside].max()) if bool(inside.any()) else 0
+    max_s = max(int(n_sent[inside].max()) if bool(inside.any()) else 1, 1)
+
+    def dv(x, dtype):
+        return torch.as_tensor(x).to(device=dev, dtype=dtype).contiguous()
+
+    with torch.cuda.device(dev):
+        d_sp, d_tp = dv(sp, torch.int64), dv(tp, torch.int64)
+        d_tok, d_chars = dv(tokens, torch.int32), dv(sent_chars, torch.int64)
+        d_ctx, d_qp, d_qt = dv(ctx_chars, torch.int64), dv(q_ptr, torch.int64), dv(q_tokens, torch.int32)
+        n_total = int(tp.numel() - 1)
+        sdt = torch.float64 if bm25_type == 0 else torch.float32
+        out = Extract(torch.empty(n_total, dtype=torch.uint8, device=dev), torch.empty(G, dtype=torch.int32, device=dev),
+                      torch.empty(n_total, dtype=sdt, device=dev) if scores else None)
+        if bm25_type == 0:
+            tab, off = _log_half(max_s + 1, dev), None
+        else:
+            tab = _bm25s_idf_table(max_s, dev)
+            off = dv(n_sent * (n_sent + 1) // 2, torch.int64)
+        if G:
+            _lib.check(_lib.lib().ezr_bm25_extract(
+                _lib.ptr(d_sp), _lib.ptr(d_tp), _lib.ptr(d_tok), int(vocab), _lib.ptr(d_chars), _lib.ptr(d_ctx),
+                _lib.ptr(d_qp), _lib.ptr(d_qt), G, max_t, max_s, _lib.ptr(tab), tab.numel(), _lib.ptr(off), k1, b,
+                epsilon, rate, _lib.F64 if bm25_type == 0 else _lib.F32, _lib.ptr(out.scores), _lib.ptr(out.keep),
+                _lib.ptr(out.counts), _lib.stream_ptr(stream)), "ezr_bm25_extract")
+        over_ids = torch.nonzero(over).flatten().tolist()
+        if over_ids:
+            qp = torch.as_tensor(q_ptr).to(torch.int64).cpu()
+            chars_h = torch.as_tensor(sent_chars).to(torch.int64).cpu().numpy()
+            ctx_h = torch.as_tensor(ctx_chars).to(torch.int64).cpu().numpy()
+            for g in over_ids:
+                s_lo, s_hi = int(sp[g]), int(sp[g + 1])
+                t_lo, t_hi = int(tp[s_lo]), int(tp[s_hi])
+                stats = Bm25Stats.from_tokens(d_tok[t_lo:t_hi], d_tp[s_lo:s_hi + 1] - t_lo, int(vocab),
+                                              bm25_type=bm25_type, k1=k1, b=b, epsilon=epsilon, device=dev)
+                index = Bm25Index(stats, device=dev, k1=k1, b=b, packed=False)
+                q = d_qt[int(qp[g]):int(qp[g + 1])]
+                row = bm25_scores(index, torch.tensor([0, q.numel()], dtype=torch.int32), q, stream=stream)[0]
+                keep = _select_host(row.cpu().numpy(), chars_h[s_lo:s_hi], int(ctx_h[g]), rate)
+                out.keep[s_lo:s_hi].copy_(torch.from_numpy(keep))
+                out.counts[g] = int(keep.sum())
+                if scores:
+                    out.scores[s_lo:s_hi].copy_(row)
     return out
 
 

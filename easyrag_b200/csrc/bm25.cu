@@ -22,6 +22,7 @@
 //    float32) of the surviving candidates only.
 // Score vectors never touch HBM on the fused paths.
 #include "ezr_common.cuh"
+#include "bm25_common.cuh"
 #include "select.cuh"
 #include "../../include/easyrag_b200.h"
 
@@ -32,10 +33,7 @@ __global__ void bm25_doc_norm_kernel(const int32_t* __restrict__ doc_len, int64_
                                      double one_minus_b, double avgdl, double* __restrict__ kd) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const double t1 = __dmul_rn(b, (double)doc_len[i]);
-    const double t2 = __ddiv_rn(t1, avgdl);
-    const double t3 = __dadd_rn(one_minus_b, t2);
-    kd[i] = __dmul_rn(k1, t3);
+    kd[i] = bm25_doc_norm((double)doc_len[i], k1, b, one_minus_b, avgdl);
 }
 
 template <typename S>
@@ -51,11 +49,7 @@ __global__ void bm25_weights_kernel(const int64_t* __restrict__ indptr, const in
         const int mid = lo + ((hi - lo) >> 1);
         if (indptr[mid] <= p) lo = mid; else hi = mid;
     }
-    const double tf = (double)post_tf[p];
-    const double num = __dmul_rn(tf, num_scale);
-    const double den = __dadd_rn(tf, kd[post_doc[p]]);
-    const double r = __ddiv_rn(num, den);
-    out_w[p] = (S)__dmul_rn(idf[lo], r);
+    out_w[p] = (S)bm25_contribution(idf[lo], (double)post_tf[p], kd[post_doc[p]], num_scale);
 }
 
 __global__ void bm25_range_index_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ post_doc,

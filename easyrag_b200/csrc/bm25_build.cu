@@ -19,6 +19,7 @@
 //   4. bm25_shard_*             a row shard's postings are a contiguous sub-segment of every term's list: two binary
 //                               searches per term, a scan, one copy (global idf / avgdl stay global, SURVEY.md 8(e)).
 #include "ezr_common.cuh"
+#include "bm25_common.cuh"
 #include "../../include/easyrag_b200.h"
 
 namespace ezr {
@@ -26,22 +27,6 @@ namespace ezr {
 constexpr int kBuildThreads = 256;
 constexpr int kBuildCap = 8192;          // tokens of a document sorted in shared memory (64 KB of 64-bit keys)
 constexpr int kBuildBlock = 8192;        // documents per placement block (independent of the query-time range)
-
-__device__ __forceinline__ void bitonic_sort_u64(unsigned long long* key, int n_pow2, int tid, int nthreads) {
-    for (int k = 2; k <= n_pow2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = tid; i < n_pow2; i += nthreads) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const unsigned long long a = key[i], b = key[ixj];
-                    const bool up = (i & k) == 0;
-                    if ((a > b) == up) { key[i] = b; key[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
 
 // status[0] != 0: a token id outside [0, vocab) was seen (its document index + 1)
 // LONG = false: documents of at most kBuildCap tokens, keys in shared memory; longer ones are skipped.

@@ -28,6 +28,11 @@ from . import _lib
 K1, B, EPSILON = 1.5, 0.75, 0.25     # retrievers.py:103-105
 
 
+def bm25s_idf(n_docs: int, df: int) -> float:
+    """bm25s' idf of a term found in ``df`` of ``n_docs`` documents, in float64 (indexes store its float32)."""
+    return math.log(1 + (n_docs - df + 0.5) / (df + 0.5))
+
+
 @dataclass
 class Bm25Stats:
     n_docs: int
@@ -124,8 +129,7 @@ class Bm25Stats:
                 neg = present[vals < 0]
                 idf[neg] = epsilon * average_idf
         elif bm25_type == 1:
-            vals = np.array([math.log(1 + (n - int(d) + 0.5) / (int(d) + 0.5)) for d in df_host[present]],
-                            dtype=np.float64).astype(np.float32)
+            vals = np.array([bm25s_idf(n, int(d)) for d in df_host[present]], dtype=np.float64).astype(np.float32)
             idf[present] = vals.astype(np.float64)
         else:
             raise ValueError("bm25_type must be 0 (BM25Okapi) or 1 (bm25s)")

@@ -183,6 +183,28 @@ int ezr_bm25_topk(const ezr_bm25_index* index, const int32_t* q_ptr, const int32
 int ezr_bm25_scores(const ezr_bm25_index* index, const int32_t* q_ptr, const int32_t* q_terms,
                     int32_t n_queries, void* out_scores, void* stream);
 
+/* ---- BM25-Extract context compression (the reference's ContextCompressor, compressors.py:32-55) ----
+ * G groups in one launch.  Group g is a context's sentences [sent_ptr[g], sent_ptr[g+1]) (tokens of sentence s:
+ * tokens[tok_ptr[s] .. tok_ptr[s+1]), ids in [0, vocab) shared by the whole batch) and its query
+ * q_tokens[q_ptr[g] .. q_ptr[g+1]) (a negative id = not in the vocabulary).  Each group is scored as if a throw-away
+ * index were built over its own sentences (BM25Retriever.get_scores(query, docs), bit for bit), the sentences are
+ * ordered by score descending then index descending, and out_keep[s] = 1 for the leading entries up to and
+ * including the first whose running sum of sent_chars is >= ctx_chars[g] * rate (all of them if none is).
+ *   score_type EZR_F64: idf_tab = double L[j] = log(j + 0.5) for j < idf_len, idf_len > max_sents; idf_off unused.
+ *   score_type EZR_F32: idf_tab = float bm25s idf; the group of N sentences reads idf_tab[idf_off[g] + df], df <= N.
+ * out_scores [S] (double / float, may be NULL), out_keep [S], out_counts[g] = number kept, or -1 for a group with no
+ * sentences, or -2 for a group with bad input (a token id out of range, more than max_tokens tokens or max_sents
+ * sentences, an idf table that does not cover it); such groups write nothing else.
+ * max_tokens / max_sents: the largest group of the batch; they size shared memory and may not exceed the caps of
+ * ezr_bm25_extract_caps (larger groups need a throw-away index and ezr_bm25_scores).  No workspace, no synchronisation. */
+int ezr_bm25_extract_caps(int32_t* max_tokens_host, int32_t* max_sents_host);
+int ezr_bm25_extract(const int64_t* sent_ptr, const int64_t* tok_ptr, const int32_t* tokens, int32_t vocab,
+                     const int64_t* sent_chars, const int64_t* ctx_chars, const int64_t* q_ptr,
+                     const int32_t* q_tokens, int32_t n_groups, int32_t max_tokens, int32_t max_sents,
+                     const void* idf_tab, int64_t idf_len, const int64_t* idf_off, double k1, double b,
+                     double epsilon, double rate, int32_t score_type, void* out_scores, uint8_t* out_keep,
+                     int32_t* out_counts, void* stream);
+
 /* ------------------------------------------------------- generic top-k --
  * Row-wise top-k of a score matrix (k <= 1024): scores[q*row_stride + j], j < n_cols.
  * positive_only != 0 keeps only scores > 0 (BM25Retriever.filter). */
