@@ -126,6 +126,8 @@ SIGNATURES = {
                                        _p]),
     "ezr_cross_pair_scores": (C.c_int, [_p, _i32, _i32, _p, C.c_float, _p, _p]),
     "ezr_cross_order_topk": (C.c_int, [_p, _p, _i32, _i32, _p, _i32, _i32, _p, _p, _p, _p, _p]),
+    "ezr_pair_union": (C.c_int, [_p, _p, _i32, _i32, _p, _p, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
+    "ezr_cross_order_topk_mapped": (C.c_int, [_p, _p, _i32, _i32, _p, _i32, _p, _i32, _i32, _p, _p, _p, _p, _p]),
     "ezr_bert_embed_typed": (C.c_int, [_p, _p, _p, _i32, _p, _p, _p, _i32, _p, _p, C.c_float, _i32, _i32, _i32, _p,
                                        _p]),
     "ezr_fuse_lists": (C.c_int, [_i32, _i32, _p, _p, _p, _i32, _i32, _p, _i32, _i32, _i32, _p, _p, _p, _p]),

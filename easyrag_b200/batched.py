@@ -432,6 +432,43 @@ def rrf_fuse(ids_a: torch.Tensor, cnt_a: torch.Tensor, ids_b: torch.Tensor, cnt_
     return out
 
 
+MAX_UNION = 1024           # k_a + k_b of ezr_pair_union: the pair packer's and the reranker head's per-query limit
+
+
+@dataclass
+class PairUnion:
+    ids: torch.Tensor        # [Q, k_a + k_b] int32: distinct ids of list a then list b, first appearance; -1 padded
+    counts: torch.Tensor     # [Q] int32
+    map_a: torch.Tensor      # [Q, k_a] int32: union index of each list-a slot, -1 past its count
+    map_b: torch.Tensor      # [Q, k_b] int32
+
+
+def pair_union(ids_a: torch.Tensor, cnt_a: torch.Tensor, ids_b: torch.Tensor, cnt_b: torch.Tensor,
+               stream=None) -> PairUnion:
+    """The per-query union of two candidate lists by document id (``ezr_pair_union``): list a = sparse, b = dense, the
+    order of ``rrf_fuse``.  ``ids_x`` int32 [Q, k_x] on the device (row stride may exceed k_x), ``cnt_x`` [Q]."""
+    if ids_a.dim() != 2 or ids_b.dim() != 2:
+        raise ValueError("ids_a and ids_b must be [Q, k]")
+    (nq, ka), (nqb, kb) = ids_a.shape, ids_b.shape
+    if nqb != nq or cnt_a.numel() != nq or cnt_b.numel() != nq:
+        raise ValueError(f"list a has {nq} queries ({cnt_a.numel()} counts), list b {nqb} ({cnt_b.numel()} counts)")
+    if ka < 1 or kb < 1 or ka + kb > MAX_UNION:
+        raise ValueError(f"k_a={ka}, k_b={kb}: each must be >= 1 and k_a + k_b <= {MAX_UNION}")
+    L = _lib.lib()
+    dev = ids_a.device
+    ids_a, ids_b = (t.to(torch.int32) for t in (ids_a, ids_b))
+    ids_a, ids_b = (t if t.stride(1) == 1 and t.stride(0) >= t.shape[1] else t.contiguous() for t in (ids_a, ids_b))
+    cnt_a, cnt_b = _i32(cnt_a, dev), _i32(cnt_b, dev)
+    out = PairUnion(torch.empty(nq, ka + kb, dtype=torch.int32, device=dev), torch.empty(nq, dtype=torch.int32, device=dev),
+                    torch.empty(nq, ka, dtype=torch.int32, device=dev), torch.empty(nq, kb, dtype=torch.int32, device=dev))
+    with torch.cuda.device(dev):
+        _lib.check(L.ezr_pair_union(_lib.ptr(ids_a), _lib.ptr(cnt_a), ka, ids_a.stride(0), _lib.ptr(ids_b),
+                                    _lib.ptr(cnt_b), kb, ids_b.stride(0), nq, _lib.ptr(out.ids), _lib.ptr(out.counts),
+                                    _lib.ptr(out.map_a), _lib.ptr(out.map_b), _lib.stream_ptr(stream)),
+                   "ezr_pair_union")
+    return out
+
+
 def _device_canon(canon: Optional[torch.Tensor], dev) -> Optional[torch.Tensor]:
     """The kernels read ``canon`` on the device: a host tensor is copied over (a host address is not valid there)."""
     return None if canon is None else canon.to(device=dev, dtype=torch.int32).contiguous()

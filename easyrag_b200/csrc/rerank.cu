@@ -10,12 +10,10 @@
 // The same head also runs in two launches (ezr_cross_pair_scores, then ezr_cross_order_topk) with a [P] fp32 score
 // vector between them; both forms share the per-pair and per-query device functions, so their outputs are identical.
 #include "ezr_common.cuh"
+#include "rerank_common.cuh"
 #include "../../include/easyrag_b200.h"
 
 namespace ezr {
-
-constexpr int kCrossThreads = 256;
-constexpr int kCrossMaxK = 1024;
 
 __device__ __forceinline__ float cross_warp_sum(float v) {
 #pragma unroll
@@ -31,33 +29,6 @@ __device__ __forceinline__ float cross_pair_sigmoid(const __nv_bfloat16* __restr
     for (int i = lane; i < dim; i += 32) acc = fmaf(tanhf(__bfloat162float(row[i])), w_out[i], acc);
     acc = cross_warp_sum(acc);
     return 1.f / (1.f + expf(-(acc + b_out)));
-}
-
-// Query q's order, by the whole CTA, from its n scores in s_sc (n <= k): every score to out_all (-inf past n), the
-// top_n by counting -- score descending, then coarse rank ascending -- to out_scores / out_ids (-inf / -1 padded).
-__device__ __forceinline__ void cross_order_write(const float* s_sc, int q, int n, int k,
-                                                  const int32_t* __restrict__ cand_ids, int k_stride, int top_n,
-                                                  float* __restrict__ out_all, float* __restrict__ out_scores,
-                                                  int32_t* __restrict__ out_ids, int32_t* __restrict__ out_counts) {
-    for (int r = threadIdx.x; r < k; r += kCrossThreads) out_all[(int64_t)q * k + r] = r < n ? s_sc[r] : -INFINITY;
-    for (int r = threadIdx.x; r < n; r += kCrossThreads) {
-        const float sr = s_sc[r];
-        int pos = 0;
-        for (int j = 0; j < n; ++j) {
-            const float sj = s_sc[j];
-            pos += (sj > sr || (sj == sr && j < r)) ? 1 : 0;       // stable descending
-        }
-        if (pos < top_n) {
-            out_scores[(int64_t)q * top_n + pos] = sr;
-            out_ids[(int64_t)q * top_n + pos] = cand_ids[(int64_t)q * k_stride + r];
-        }
-    }
-    const int c = min(n, top_n);
-    for (int i = c + threadIdx.x; i < top_n; i += kCrossThreads) {
-        out_scores[(int64_t)q * top_n + i] = -INFINITY;
-        out_ids[(int64_t)q * top_n + i] = -1;
-    }
-    if (threadIdx.x == 0) out_counts[q] = c;
 }
 
 __global__ void __launch_bounds__(kCrossThreads)

@@ -13,7 +13,8 @@ sorted per-shard lists by rank (``ezr_merge_sorted_parts``).
 
 Fine ranking (:class:`ShardedCrossEncoderReranker`) splits the other way: every rank holds the whole cross-encoder and
 the same candidate lists, the (query, candidate) pairs are cut into token-balanced runs, one per rank, and ONE
-all-reduce of a [P] fp32 score vector gives every rank every pair's score; each rank then orders all queries.
+all-reduce of a [P] fp32 score vector gives every rank every pair's score; each rank then orders all queries.  Its
+``rerank_fusion`` splits the pairs of the union of two candidate lists the same way.
 """
 from __future__ import annotations
 
@@ -437,3 +438,29 @@ class ShardedCrossEncoderReranker:
                                               _lib.stream_ptr()), "ezr_cross_order_topk")
             _mark(events)
         return out, all_scores
+
+    def rerank_fusion(self, sparse, dense, q_ptr: torch.Tensor, q_tok: torch.Tensor, top_n: int, k_out: int,
+                      K: int = 60, canon: Optional[torch.Tensor] = None,
+                      events: Optional[List[torch.cuda.Event]] = None):
+        """Same arguments and result as ``CrossEncoderReranker.rerank_fusion``, bit-identical to it: every rank builds
+        and packs the union of the two lists, encodes its token-balanced run of the union's pairs, and after one
+        :func:`exchange_pair_scores` orders both routes and fuses them.  The cross-rank check covers both list shapes
+        and the union's pair and token totals.  Stage events as in :meth:`rerank`."""
+        from .rerank import _mark
+        rr = self.reranker
+        _mark(events)
+        union, pairs = rr._union_pack(sparse, dense, q_ptr, q_tok, top_n, k_out)
+        if self.distributed:
+            check_replicated((pairs.n_queries, union.map_a.shape[1], union.map_b.shape[1], pairs.n_pairs,
+                              int(pairs.cu_h[-1])), "list shapes [Q, k_sparse], [Q, k_dense], union pair and token "
+                             "totals", self.group, self._check_device)
+        _mark(events)
+        lo, hi = token_balanced_ranges(pairs.cu_h, self.world)[self.rank]
+        sig = torch.zeros(pairs.n_pairs, dtype=torch.float32, device=rr.device)
+        with torch.cuda.device(rr.device):
+            rr._score_run(pairs, lo, hi, sig, events)
+            if self.distributed and pairs.n_pairs:
+                exchange_pair_scores(sig, self.group)
+            out = rr._fusion_orders(sig, pairs, union, sparse, dense, top_n, k_out, K, canon)
+            _mark(events)
+        return out

@@ -9,7 +9,8 @@ by ``sorted(nodes, key=lambda x: -x.score if x.score else 0)``.  Here:
 * ``CrossEncoderReranker``  - the batched device path: a ``[Q, k]`` ``TopK`` of the coarse ranker -> the pairs packed
   on the device from passages tokenised once (csrc/handoff.cu), the encoder run in chunks of whole pairs under a
   token budget, the CLS rows through Linear + bias (ezr_pool_normalize + ezr_gemm_bf16), then tanh / dot / sigmoid
-  and the per-query order in one kernel (csrc/rerank.cu).
+  and the per-query order in one kernel (csrc/rerank.cu).  ``rerank_fusion`` reranks a sparse and a dense list
+  separately and fuses them by RRF (pipeline.py:393-452), encoding the pairs of both lists once (csrc/rerank_fusion.cu).
 * ``SentenceTransformerRerank`` - the drop-in node postprocessor, built on the batched path with one query.
 """
 from __future__ import annotations
@@ -126,6 +127,23 @@ class CrossPairs:
         return self.cu_h.size - 1
 
 
+@dataclass
+class RerankFusion:
+    """Result of :meth:`CrossEncoderReranker.rerank_fusion`: each route reranked on its own, and the two fused."""
+    fused: TopK                # [Q, k_out], float64 RRF scores of the two reranked top_n lists (sparse first on ties)
+    sparse: TopK               # [Q, top_n], float32 sigmoid scores, as ``rerank`` returns for the sparse list
+    dense: TopK                # [Q, top_n]
+    sparse_all: torch.Tensor   # float32 [Q, k_sparse], -inf padded
+    dense_all: torch.Tensor    # float32 [Q, k_dense]
+    n_pairs: int               # distinct (query, passage) pairs encoded
+    route_pairs: torch.Tensor  # int64 [] on the device: the pairs of both routes, read by ``n_route_pairs``
+
+    @property
+    def n_route_pairs(self) -> int:
+        """The pairs two ``rerank`` calls would encode (reading it synchronises with the device)."""
+        return int(self.route_pairs)
+
+
 class CrossEncoderReranker:
     """Batched fine ranking of coarse candidate lists on the GPU.
 
@@ -232,6 +250,76 @@ class CrossEncoderReranker:
                        "ezr_cross_score_topk")
             _mark(events)
         return out, all_scores
+
+    def rerank_fusion(self, sparse: TopK, dense: TopK, q_ptr: torch.Tensor, q_tok: torch.Tensor, top_n: int,
+                      k_out: int, K: int = 60, canon: Optional[torch.Tensor] = None,
+                      events: Optional[List[torch.cuda.Event]] = None) -> RerankFusion:
+        """``generation_with_rerank_fusion`` (pipeline.py:393-452) for a batch: the sparse and the dense coarse lists
+        (ids int32 [Q, k_sparse] / [Q, k_dense], -1 padded, and counts [Q]) each reranked to ``top_n``, then
+        ``rrf_fuse(sparse, dense)`` to ``k_out`` (``canon``: as in ``rrf_fuse``).  Every output is bit-identical to two
+        :meth:`rerank` calls and ``rrf_fuse``, but a document in both lists is packed and encoded once: the pairs are
+        those of ``batched.pair_union`` (one pack, one encoder run, one head), and each route is ordered from the
+        union's scores through its slot map.  k_sparse + k_dense <= 1024.  ``events``: as in :meth:`rerank` (the
+        union is in the first stage)."""
+        _mark(events)
+        union, pairs = self._union_pack(sparse, dense, q_ptr, q_tok, top_n, k_out)
+        _mark(events)
+        sig = torch.empty(pairs.n_pairs, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            self._score_run(pairs, 0, pairs.n_pairs, sig, events)
+            out = self._fusion_orders(sig, pairs, union, sparse, dense, top_n, k_out, K, canon)
+            _mark(events)
+        return out
+
+    def _union_pack(self, sparse: TopK, dense: TopK, q_ptr: torch.Tensor, q_tok: torch.Tensor, top_n: int,
+                    k_out: int):
+        """The checks of :meth:`rerank_fusion`, the union of the two lists and its pack -> (PairUnion, CrossPairs)."""
+        from .batched import pair_union
+        if top_n < 1 or k_out < 1:
+            raise ValueError(f"top_n={top_n} and k_out={k_out} must be >= 1")
+        dev = self.device
+        union = pair_union(sparse.ids.to(dev), sparse.counts.to(dev), dense.ids.to(dev), dense.counts.to(dev))
+        return union, self.pack(union.ids, union.counts, q_ptr, q_tok)
+
+    def _score_run(self, pairs: CrossPairs, lo: int, hi: int, sig: torch.Tensor,
+                   events: Optional[List[torch.cuda.Event]]) -> None:
+        """Pairs [lo, hi) through the chunked encoder (then an event), Linear + bias and the sigmoid into sig[lo:hi]."""
+        m, d = self.model, self.model.cfg.hidden_size
+        if hi > lo:
+            cls = torch.empty(hi - lo, d, dtype=torch.bfloat16, device=self.device)
+            for p0, p1 in self.chunks(pairs.cu_h[lo:hi + 1]):
+                self._encode_cls(pairs, lo + p0, lo + p1, cls[p0:p1])
+        _mark(events)
+        if hi > lo:
+            rows = gemm(cls, m.w1, bias=m.b1)
+            _lib.check(_lib.lib().ezr_cross_pair_scores(_lib.ptr(rows), d, hi - lo, _lib.ptr(m.w2), m.b2,
+                                                        _lib.ptr(sig[lo:hi]), _lib.stream_ptr()),
+                       "ezr_cross_pair_scores")
+
+    def _fusion_orders(self, sig: torch.Tensor, pairs: CrossPairs, union, sparse: TopK, dense: TopK, top_n: int,
+                       k_out: int, K: int, canon: Optional[torch.Tensor]) -> RerankFusion:
+        """Both routes ordered from the union's pair scores ``sig`` (``ezr_cross_order_topk_mapped``), then RRF."""
+        from .batched import rrf_fuse
+        L, dev, nq = _lib.lib(), self.device, pairs.n_queries
+        routes = []
+        for cand, slot_map in ((sparse, union.map_a), (dense, union.map_b)):
+            ids = cand.ids.to(device=dev, dtype=torch.int32)
+            if ids.stride(1) != 1:
+                ids = ids.contiguous()
+            k = ids.shape[1]
+            top = TopK(torch.empty(nq, top_n, dtype=torch.float32, device=dev),
+                       torch.empty(nq, top_n, dtype=torch.int32, device=dev),
+                       torch.empty(nq, dtype=torch.int32, device=dev))
+            all_scores = torch.empty(nq, k, dtype=torch.float32, device=dev)
+            _lib.check(L.ezr_cross_order_topk_mapped(_lib.ptr(sig), _lib.ptr(pairs.pair_off), nq, k, _lib.ptr(slot_map),
+                                                     slot_map.stride(0), _lib.ptr(ids), ids.stride(0), top_n,
+                                                     _lib.ptr(all_scores), _lib.ptr(top.scores), _lib.ptr(top.ids),
+                                                     _lib.ptr(top.counts), _lib.stream_ptr()),
+                       "ezr_cross_order_topk_mapped")
+            routes.append((top, all_scores, cand.counts.to(dev).clamp(0, k).sum()))
+        (s, s_all, s_n), (d, d_all, d_n) = routes
+        fused = rrf_fuse(s.ids, s.counts, d.ids, d.counts, k_out, K=K, canon=canon)
+        return RerankFusion(fused, s, d, s_all, d_all, pairs.n_pairs, s_n + d_n)
 
     def chunks(self, cu_h: np.ndarray) -> List[Tuple[int, int]]:
         """Consecutive runs [p0, p1) of whole pairs holding at most ``max_tokens`` tokens and at most

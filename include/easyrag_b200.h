@@ -420,6 +420,26 @@ int ezr_cross_pair_scores(const void* dense, int32_t dim, int32_t n_pairs, const
 int ezr_cross_order_topk(const float* sig, const int32_t* pair_off, int32_t n_queries, int32_t k,
                          const int32_t* cand_ids, int32_t k_stride, int32_t top_n, float* out_all, float* out_scores,
                          int32_t* out_ids, int32_t* out_counts, void* stream);
+/* Rerank fusion (generation_with_rerank_fusion, pipeline.py:393-452): two coarse lists per query reranked separately,
+ * their pairs packed and encoded once as the union of the two lists.
+ * pair_union:  per query, the distinct DOCUMENT ids (not canon keys: the reranker scores each id's own passage) of
+ *              list a's slots [0, cnt_a) then list b's [0, cnt_b), in first-appearance order -- the lists disjoint,
+ *              that is list a followed by list b.  out_ids int32 [Q, k_a + k_b] (-1 past the count), out_counts [Q],
+ *              out_map_a [Q, k_a] / out_map_b [Q, k_b] the union index of every list slot (-1 past the list's count).
+ *              Each list holds distinct ids (a coarse top-k); a repeated id maps its slots to one union entry.
+ *              Counts are clamped to [0, k].  k_a + k_b <= 1024, else EZR_ERR_INVALID.  One CTA per query.
+ * order_topk_mapped: ezr_cross_order_topk for one list from the union's scores: sig float32 [P] holds the union's
+ *              pairs (pair pair_off[q] + u = union entry u of query q), slot_map [Q][map_stride] the list's map
+ *              (pair_union's out_map_x); list slot r scores sig[pair_off[q] + slot_map[q, r]].  The list's count is
+ *              the map's leading run of entries in [0, pair count of q).  Outputs and order are those of
+ *              ezr_cross_order_topk on the list alone (cand_ids / k_stride: the list's ids).  k <= 1024. */
+int ezr_pair_union(const int32_t* ids_a, const int32_t* cnt_a, int32_t k_a, int32_t stride_a, const int32_t* ids_b,
+                   const int32_t* cnt_b, int32_t k_b, int32_t stride_b, int32_t n_queries, int32_t* out_ids,
+                   int32_t* out_counts, int32_t* out_map_a, int32_t* out_map_b, void* stream);
+int ezr_cross_order_topk_mapped(const float* sig, const int32_t* pair_off, int32_t n_queries, int32_t k,
+                                const int32_t* slot_map, int32_t map_stride, const int32_t* cand_ids, int32_t k_stride,
+                                int32_t top_n, float* out_all, float* out_scores, int32_t* out_ids,
+                                int32_t* out_counts, void* stream);
 
 /* ------------------------------------------------------------ encoder ---
  * Building blocks of the chunk/query embedding forward pass (GTEEmbedding._embed, gte_embeddings.py:59-72 ->
