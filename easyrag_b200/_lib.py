@@ -132,6 +132,15 @@ SIGNATURES = {
                                        _p]),
     "ezr_fuse_lists": (C.c_int, [_i32, _i32, _p, _p, _p, _i32, _i32, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
     "ezr_fusion_simple": (C.c_int, [_p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i32, _p, _p, _p, _p]),
+    "ezr_vocab_set_hash_bits": (C.c_int, [_i32]),
+    "ezr_vocab_table_bytes": (_sz, [_i64]),
+    "ezr_vocab_workspace": (_sz, [_i64, _i64]),
+    "ezr_vocab_table_init": (C.c_int, [_p, _i64, _p]),
+    "ezr_vocab_table_grow": (C.c_int, [_p, _i64, _p, _i64, _p]),
+    "ezr_vocab_insert": (C.c_int, [_p, _i64, _p, _i64, _i64, _i64, _p, _i64, _p, _p, _i64, C.POINTER(C.c_int64), _p,
+                                   _p, _p, _sz, _p]),
+    "ezr_vocab_lookup": (C.c_int, [_p, _i64, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "ezr_vocab_read": (C.c_int, [_p, _p, _i64, _i64, _p, _sz, C.POINTER(C.c_int64), _p]),
 }
 
 _lib = None

@@ -8,8 +8,9 @@ until their characters reach ``rate * len(context)`` and joins the kept ones in 
 (csrc/bm25_extract.cu): every context is one group, scored bit for bit as ``get_scores(query, sentences)`` scores it.
 
 Host work that stays in Python: sentence splitting (the reference's own ``cut_sent`` unless a ``splitter`` is given),
-tokenisation with the retriever's tokenizer and stop words (as ``get_scores`` does), packing the batch into CSR
-arrays over one vocabulary, and joining the kept sentences.
+tokenisation with the retriever's tokenizer and stop words (as ``get_scores`` does) and joining the kept sentences.
+``compress_batch`` packs the batch into CSR arrays over one vocabulary on the device (:func:`pack_device`, through
+:class:`easyrag_b200.vocab.Vocabulary`); :func:`pack` is the same packing as a host loop.
 
 Ties between equal scores are broken by sentence index, higher first (the project's canonical order); the
 reference's ``argsort()[::-1]`` leaves that order to numpy's unstable sort.
@@ -17,13 +18,14 @@ reference's ``argsort()[::-1]`` leaves that order to numpy's unstable sort.
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence, Union
 
 import numpy as np
 import torch
 
 from . import batched
 from .retrievers import BM25Retriever, tokenize_and_remove_stopwords
+from .vocab import Vocabulary
 
 
 def _reference_cut_sent() -> Callable[[str], List[str]]:
@@ -44,7 +46,8 @@ def split_sentences(context: str, splitter: Callable[[str], List[str]]) -> List[
 class Packed:
     """A batch of groups over one vocabulary (CSR, host arrays): sentences ``sent_ptr[g]:sent_ptr[g+1]``, tokens of
     sentence s ``tokens[tok_ptr[s]:tok_ptr[s+1]]``, query tokens ``q_tokens[q_ptr[g]:q_ptr[g+1]]`` (-1 = no sentence of
-    the batch has it), character counts of every sentence and context."""
+    the batch has it), character counts of every sentence and context.  From :func:`pack_device`, ``tokens`` and
+    ``q_tokens`` are int32 device tensors and ``vocab`` is a :class:`~easyrag_b200.vocab.Vocabulary`."""
     sent_ptr: np.ndarray     # int64 [G+1]
     tok_ptr: np.ndarray      # int64 [S+1]
     tokens: np.ndarray       # int32 [T]
@@ -52,7 +55,7 @@ class Packed:
     ctx_chars: np.ndarray    # int64 [G]
     q_ptr: np.ndarray        # int64 [G+1]
     q_tokens: np.ndarray     # int32
-    vocab: Dict[str, int]
+    vocab: Union[Dict[str, int], Vocabulary]     # pack: the dict; pack_device: the device vocabulary
 
 
 def pack(query_tokens: Sequence[Sequence[str]], sentence_tokens: Sequence[Sequence[Sequence[str]]],
@@ -76,6 +79,20 @@ def pack(query_tokens: Sequence[Sequence[str]], sentence_tokens: Sequence[Sequen
                   sent_chars=np.asarray([len(s) for sents in sentences for s in sents], dtype=np.int64),
                   ctx_chars=np.asarray([len(c) for c in contexts], dtype=np.int64),
                   q_ptr=np.asarray(q_ptr, dtype=np.int64), q_tokens=np.asarray(q_flat, dtype=np.int32), vocab=vocab)
+
+
+def pack_device(query_tokens: Sequence[Sequence[str]], sentence_tokens: Sequence[Sequence[Sequence[str]]],
+                sentences: Sequence[Sequence[str]], contexts: Sequence[str], device="cuda") -> Packed:
+    """:func:`pack` with the term ids made on the device: the same ids, with ``tokens`` and ``q_tokens`` left there for
+    :func:`easyrag_b200.batched.bm25_extract`.  Pointers and character counts stay on the host."""
+    vocab = Vocabulary(device)
+    tokens, tok_ptr = vocab.intern([toks for sents in sentence_tokens for toks in sents])
+    q_tokens, q_ptr = vocab.lookup(query_tokens)
+    return Packed(sent_ptr=np.concatenate([[0], np.cumsum([len(s) for s in sentence_tokens])]).astype(np.int64),
+                  tok_ptr=tok_ptr.numpy(), tokens=tokens,
+                  sent_chars=np.asarray([len(s) for sents in sentences for s in sents], dtype=np.int64),
+                  ctx_chars=np.asarray([len(c) for c in contexts], dtype=np.int64),
+                  q_ptr=q_ptr.numpy(), q_tokens=q_tokens, vocab=vocab)
 
 
 class ContextCompressor:
@@ -117,7 +134,7 @@ class ContextCompressor:
                     for q, s, c in zip(queries, sentences, contexts)]
             return self.join(sentences, np.concatenate(keep))
         q_toks, s_toks = self.tokenize(queries, sentences)
-        keep, _ = self.run(pack(q_toks, s_toks, sentences, contexts))
+        keep, _ = self.run(pack_device(q_toks, s_toks, sentences, contexts, r.bm25.device))
         return self.join(sentences, keep)
 
     # ---- the steps of compress_batch, separately callable (scripts/bench_compress.py times each)

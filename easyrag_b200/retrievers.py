@@ -22,6 +22,7 @@ from . import _lib, batched
 from .index import Bm25Index, Bm25Stats, DenseIndex, K1, B, EPSILON, normalize_rows
 from .schema import (BaseEmbedding, BaseNode, BaseRetriever, NodeWithScore, QueryBundle, VectorStoreQuery,
                      VectorStoreQueryResult, filter_conditions)
+from .vocab import Vocabulary
 
 logger = logging.getLogger(__name__)
 
@@ -309,13 +310,16 @@ class BM25Retriever(BaseRetriever):
         self.bm25_type = bm25_type
         self.k1, self.b, self.epsilon = K1, B, EPSILON
         self._device = device
-        self._vocab, tokens, doc_ptr = _encode_corpus(self._corpus)
+        # the corpus is interned on the device (easyrag_b200.vocab): the same ids and dict as _encode_corpus
+        vocab = Vocabulary(device)
+        tokens, doc_ptr = vocab.intern(self._corpus)
+        self._vocab = vocab.to_dict()
         self.bm25 = self._build(tokens, doc_ptr, len(self._vocab), packed=packed)
         self.filter_dict = None
         self.stopwords = stopwords
         self._groups = _GroupTable(self._nodes)
         self._group_keys: Optional[Tuple[str, ...]] = None
-        self.canon = torch.from_numpy(_canon_ids([n.get_content() for n in self._nodes]))
+        self.canon = Vocabulary(device).first_index([n.get_content() for n in self._nodes]).to(torch.int32).cpu()
         self._ws = batched.Workspace(self.bm25.device)
         super().__init__(callback_manager=callback_manager, object_map=object_map, objects=objects, verbose=verbose)
 
@@ -331,7 +335,8 @@ class BM25Retriever(BaseRetriever):
         return ptr, ids
 
     def get_scores(self, query, docs=None):
-        """retrievers.py:128-151 -> numpy score vector (float64 for bm25_type 0, float32 for 1)."""
+        """retrievers.py:128-151 -> numpy score vector (float64 for bm25_type 0, float32 for 1).  ``docs``: one
+        context per call, small enough that its vocabulary stays a host dict (``_encode_corpus``)."""
         if docs is None:
             index, vocab = self.bm25, self._vocab
         else:

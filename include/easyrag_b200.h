@@ -524,6 +524,40 @@ int ezr_pool_normalize(const void* hidden, int64_t ldh, const int32_t* cu_seqlen
                        int32_t final_norm, const void* gamma, float eps, int32_t l2_mode, int32_t dim, void* out_bf16,
                        float* out_f32, void* stream);
 
+/* ------------------------------------------------------ string interning --
+ * csrc/vocab.cu (easyrag_b200/vocab.py, DESIGN.md §4.9): the id a Python dict filled in first-seen order gives each
+ * string (d.setdefault(s, len(d))) and the global index of its first occurrence, for chunks of n_strings UTF-8 strings
+ * joined by single NUL bytes (n_bytes bytes, exactly n_strings - 1 NULs; zero-length strings are keys too).
+ * State, all caller-owned device memory:
+ *   table     ezr_vocab_table_bytes(capacity) bytes, capacity a power of two in [2, 2^40]; it records the hash bits
+ *             in force when ezr_vocab_table_init made it, and ezr_vocab_table_grow keeps them.
+ *   arena     the bytes of every id in id order; arena_off int64 [id_capacity + 1] (arena_off[0] = 0): id i's bytes
+ *             are arena[arena_off[i] .. arena_off[i + 1]).  id_first int64 [id_capacity]: id i's first index.
+ *   state_host int64 [2] on the host: {ids, arena bytes used}; ezr_vocab_insert updates it.
+ * insert: interns the chunk (its strings have global indices first_index ..) and writes out_ids int32 [n_strings] and,
+ *   when out_first != NULL, out_first int64 [n_strings].  Needs 2 * (ids + n_strings) <= capacity (grow the table
+ *   first), else EZR_ERR_WORKSPACE.  New ids past id_capacity or new bytes past arena_capacity: EZR_ERR_WORKSPACE; an
+ *   id past INT32_MAX: EZR_ERR_INVALID; the table is then left as it was.  Synchronises the stream once.
+ * lookup: the same ids without inserting; -1 (and first index -1) for a string the table does not hold.  Synchronises.
+ * A separator count other than n_strings - 1 is EZR_ERR_INVALID and writes no output.  Chunks: n_bytes < 2^32.
+ * read: copies arena_off[id_lo .. id_hi] to off_host and the bytes of ids [id_lo, id_hi) to bytes_host (synchronises).
+ * set_hash_bits: hash bits (1..64, default 64) of tables made afterwards on this host thread; fewer bits make equal
+ *   hashes of different strings common (tests of the byte comparison).  Results are the same at every setting. */
+int ezr_vocab_set_hash_bits(int32_t bits);
+size_t ezr_vocab_table_bytes(int64_t capacity);
+size_t ezr_vocab_workspace(int64_t n_strings, int64_t n_bytes);
+int ezr_vocab_table_init(void* table, int64_t capacity, void* stream);
+int ezr_vocab_table_grow(const void* table, int64_t capacity, void* new_table, int64_t new_capacity, void* stream);
+int ezr_vocab_insert(void* table, int64_t capacity, const uint8_t* bytes, int64_t n_bytes, int64_t n_strings,
+                     int64_t first_index, uint8_t* arena, int64_t arena_capacity, int64_t* arena_off,
+                     int64_t* id_first, int64_t id_capacity, int64_t* state_host, int32_t* out_ids,
+                     int64_t* out_first, void* workspace, size_t ws_bytes, void* stream);
+int ezr_vocab_lookup(const void* table, int64_t capacity, const uint8_t* bytes, int64_t n_bytes, int64_t n_strings,
+                     const uint8_t* arena, const int64_t* arena_off, const int64_t* id_first, int32_t* out_ids,
+                     int64_t* out_first, void* workspace, size_t ws_bytes, void* stream);
+int ezr_vocab_read(const uint8_t* arena, const int64_t* arena_off, int64_t id_lo, int64_t id_hi, uint8_t* bytes_host,
+                   size_t bytes_cap, int64_t* off_host, void* stream);
+
 /* ----------------------------------------------------------- profiling ---
  * Per-kernel CUDA-event timing on the launching stream, for bench.py's roofline figures.
  * ezr_profile_read synchronises on the recorded events and returns the summed duration of the
